@@ -242,30 +242,6 @@ def test_peer_buffers_single_process(eng):
         assert (got[o:o + n + 5] == want[:n + 5]).all() and (got[o + n + 5:o + n + 8] == 0).all()
     with pytest.raises(AssertionError, match="unsupported size"):
         eng._check(eng.lib.sa_push(dsts, 3, ptrs[0], 24, eng._stream()))
-    # the other variants of the push kernel (SA_PUSH_MODE, read once per process): 1 = one destination per CTA
-    import subprocess
-    import sys
-    code = r'''
-import sys, ctypes
-sys.path[:0] = [%r]
-import torch, sa_engine
-eng = sa_engine.get_engine()
-for n in (1000, 70001):
-    src = torch.randint(0, 1 << 62, (n, 2), dtype=torch.int64, device=eng.device)
-    dst = torch.zeros((7 * (n + 3), 2), dtype=torch.int64, device=eng.device)
-    for nd in (1, 3, 7):
-        dst.zero_()
-        ptrs = (ctypes.c_void_p * nd)(*[dst.data_ptr() + 16 * (n + 3) * i for i in range(nd)])
-        eng._check(eng.lib.sa_push(ptrs, nd, src.data_ptr(), 16 * n, eng._stream()))
-        for i in range(7):
-            blk = dst[(n + 3) * i:(n + 3) * (i + 1)]
-            assert bool((blk[:n] == src).all()) == (i < nd) and int(blk[n:].abs().sum()) == 0
-print("PUSH_MODE1_OK")
-''' % os.path.join(ROOT_DIR, "stark-anatomy_b200")
-    for push_mode in ("1", "2"):  # 2 = the TMA variant (bulk-async load to shared memory, one bulk store per peer)
-        out = subprocess.run([sys.executable, "-c", code], text=True, capture_output=True, timeout=300,
-                             env=dict(os.environ, SA_PUSH_MODE=push_mode))
-        assert "PUSH_MODE1_OK" in out.stdout, push_mode + out.stdout[-500:] + out.stderr[-2000:]
     full = sa_dist.sharded_ntt(up(eng, x), 12, w, assemble="p2p-store", peers=pb)  # world 1: plain transform
     assert (down(eng, full) == want).all()
     pb.close()
@@ -724,44 +700,22 @@ def test_dropin_fri_commit_2_20_golden_roots(eng):
     C.case_fri_commit_2_20()  # BASELINE.md section 3 (73.1 s of reference time)
 
 
-def test_fri_commit_persistent_tail_opt_in(eng):
-    """SA_FRI_PERSISTENT=1: the narrow rounds of sa_fri_commit run in ONE persistent launch (the kernel waits for
-    each challenge in mapped host memory).  Off by default (the narrow rounds are hash chains, not launch overhead);
-    when on it must give the reference's transcripts, and a challenge callback that raises
-    while the kernel is waiting must abort it cleanly.  Own interpreter: the mode is decided once per process."""
-    import subprocess
-    import sys
+def test_fri_commit_callback_abort(eng):
+    """a challenge callback that raises partway through sa_fri_commit aborts the commit with its exception, and
+    later commits still give the reference's transcripts"""
+    class Boom(Exception):
+        pass
+
+    def on_root(r, root, want):
+        if r == 3:
+            raise Boom()
+        return 12345
+    n = 1 << 12
+    with pytest.raises(Boom):
+        eng.fri_commit(up(eng, rand_np(9, n)), 8, O.GENERATOR, O.primitive_nth_root(n), on_root)
+    eng.synchronize()
     C.case_fri_commit(1 << 12)
-    assert eng.lib.sa_fri_tail_mode() == 0
-    code = r'''
-import sys
-sys.path[:0] = [%r, %r, %r]
-import numpy as np, pytest
-import dropin_cases as C, sa_engine, oracle as O
-eng = sa_engine.get_engine()
-C.case_fri_commit(1 << 12)
-assert eng.lib.sa_fri_tail_mode() == 1, "the persistent tail is not active (launches serialised by a tool?)"
-C.case_fri_prove(1 << 10)
-C.case_fri_commit_2_20()
-n = 1 << 12
-rng = np.random.default_rng(9)
-cw = eng.upload(np.stack([rng.integers(0, 1 << 64, size=n, dtype=np.uint64),
-                          rng.integers(0, 0xCB80000000000000, size=n, dtype=np.uint64)], axis=1).view(np.int64))
-class Boom(Exception):
-    pass
-def on_root(r, root, want):
-    if r == 3:
-        raise Boom()
-    return 12345
-with pytest.raises(Boom):
-    eng.fri_commit(cw, 8, O.GENERATOR, O.primitive_nth_root(n), on_root)
-eng.synchronize()
-C.case_fri_commit(1 << 12)  # and the engine is still fine
-print("TAIL_OK")
-''' % (os.path.join(ROOT_DIR, "stark-anatomy_b200"), os.path.join(ROOT_DIR, "oracle"), os.path.join(ROOT_DIR, "tests"))
-    out = subprocess.run([sys.executable, "-c", code], text=True, capture_output=True, timeout=900,
-                         env=dict(os.environ, SA_FRI_PERSISTENT="1"))
-    assert "TAIL_OK" in out.stdout, out.stdout[-1000:] + out.stderr[-3000:]
+    C.case_fri_commit_2_20()
 
 
 def test_dropin_fri_prove_and_verify(eng):
