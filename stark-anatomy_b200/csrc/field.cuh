@@ -46,6 +46,10 @@ SA_HD fe fe_one() { return fe_make(1, 0, 0, 0); }
 SA_HD fe fe_mont_one() { return fe_make(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0x347FFFFFu); }  // R mod p, R = 2^128
 SA_HD fe fe_r2() { return fe_make(0x0E778236u, 0x5BD53A7Fu, 0x1A6AEDC2u, 0xAAF4AD9Au); }  // R^2 mod p
 SA_HD fe fe_from_u64(uint64_t x) { return fe_make((uint32_t)x, (uint32_t)(x >> 32), 0, 0); }
+// the C ABI's two little-endian 64-bit words
+SA_HD fe fe_from_limbs(const uint64_t x[2]) {
+    return fe_make((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
+}
 SA_HD bool fe_is_zero(const fe &a) { return (a.v[0] | a.v[1] | a.v[2] | a.v[3]) == 0; }
 SA_HD bool fe_eq(const fe &a, const fe &b) {
     return ((a.v[0] ^ b.v[0]) | (a.v[1] ^ b.v[1]) | (a.v[2] ^ b.v[2]) | (a.v[3] ^ b.v[3])) == 0;

@@ -1,7 +1,10 @@
 // fri_merkle.cuh -- per-thread pieces of the FRI round kernel: split-and-fold
 // (code/fri.py:85) and the chunked Merkle reduction (code/merkle.py:6-14).
-// __host__ __device__ so tests/emu can drive the same code phase by phase.
+// __host__ __device__ so tests/emu can drive the same code phase by phase; the launch loop of a tree
+// and the fold scalars are shared with it too.
 #pragma once
+#include <cstdio>
+
 #include "field.cuh"
 #include "hash.cuh"
 
@@ -88,6 +91,55 @@ SA_HD void merkle_shape(MerkleArgs &a) {
 }
 // width of the level a launch of shape `a` leaves behind
 SA_HD long long merkle_next_width(const MerkleArgs &a) { return a.width >> (a.ipt_log + a.red_log); }
+
+// spec = "minlog:ipt:chunklog:red:coopmax,..." (SA_MK_SHAPE with -DSA_TUNE): the row with the largest
+// minlog <= log2(width) (and chunklog <= log2(width)) replaces the launch shape of the level
+inline void merkle_shape_override(MerkleArgs &a, const char *spec) {
+    int best = -1, w = merkle_log2(a.width);
+    while (*spec) {
+        int ml, ipt, cl, red, coop, used = 0;
+        if (sscanf(spec, "%d:%d:%d:%d:%d%n", &ml, &ipt, &cl, &red, &coop, &used) != 5) break;
+        if (ml <= w && ml > best && cl <= w) {
+            best = ml;
+            a.ipt_log = ipt;
+            a.chunk = 1 << cl;
+            a.red_log = red;
+            a.coop_max = coop;
+        }
+        spec += used;
+        if (*spec == ',') spec++;
+    }
+}
+
+// Launches of one tree: the first handles the bottom level in a.mode, later ones continue from the
+// digests the previous one left.  With an arrival counter (`ticket`), the launch that leaves at most
+// MK_THREADS single-digest CTAs also reduces those; without one, that takes one more launch.
+// shape_spec (nullptr: none) goes to merkle_shape_override.  launch(a, last) runs one launch and returns
+// 0 or an error code; `last` marks the launch that finishes the tree.
+template <class Launch>
+int merkle_launches(MerkleArgs a, unsigned int *ticket, const char *shape_spec, Launch &&launch) {
+    while (true) {
+        merkle_shape(a);
+        if (shape_spec) merkle_shape_override(a, shape_spec);
+        const long long left = merkle_next_width(a), grid = a.width / a.chunk;
+        const bool fuse_top = left > 1 && left <= MK_THREADS && left == grid && ticket != nullptr;
+        const bool last = left <= 1 || fuse_top;
+        a.ticket = fuse_top ? ticket : nullptr;
+        const int rc = launch(a, last);
+        if (rc != 0 || last) return rc;
+        a.width = left;
+        a.mode = 0;
+    }
+}
+
+// the scalars of a fold (fri.py:85) in Montgomery form: inv2_m = 2^-1, s_m = alpha * 2^-1 * offset^-1.
+// oinv_m is offset^-1 in Montgomery form: a commit squares it along with offset from round to round, since
+// a Fermat inversion on the host costs ~10 us (a fifth of a round trip); 2^-1 is computed once.
+inline void fri_fold_scalars(fe *s_m, fe *inv2_m, const fe &alpha, const fe &oinv_m) {
+    static const fe inv2 = fe_mont_inv(fe_to_mont(fe_from_u64(2)));
+    *inv2_m = inv2;
+    *s_m = fe_montmul(fe_montmul(fe_to_mont(alpha), inv2), oinv_m);
+}
 
 // digest of bottom node g of this launch: loads it (mode 0) or hashes the leaf (modes 1, 2) and
 // writes it to the tree (and next[] in mode 2)

@@ -1,5 +1,6 @@
-// ntt_plan.cuh -- how an n-point transform (code/ntt.py:3-30) is cut into tile passes.
-// Shared by the CUDA host code (sa_b200.cu) and the CPU emulation (tests/emu).
+// ntt_plan.cuh -- how an n-point transform (code/ntt.py:3-30) is cut into tile passes: the roots,
+// the contents of the twiddle tables and the pass sequence.  The library (ntt.cu) runs it with
+// kernel launches, the CPU emulation (tests/emu) with loops over the kernels' phase functions.
 //
 //   log_n <= 10 : one pass, every transform is one tile column.
 //   log_n 11..20: four-step split n = n1 * n2 (n1 = 2^l1 >= n2 = 2^l2):
@@ -14,11 +15,43 @@
 //       pass 2: inside every k1 block, n2-point transforms over j2 (stride n3), times (w^n1)^(k2*j3);
 //       pass 3: n3-point transforms over j3 (contiguous), written to out[k1 + n1*k2 + n1*n2*k3].
 #pragma once
+#include <cstring>
+
+#include "../../include/sa_b200.h"
 #include "ntt_tile.cuh"
 
 namespace sa {
 
 constexpr int NTT_MAX_LOG_N = 26;  // the pass-1 twiddle matrix has n entries (1 GiB at 2^26)
+
+// Thread `thread` of a power table: out[slot(e)] = base^e * lead (Montgomery form) for its 16 consecutive
+// exponents e < count.  swz != 0 stores in the bank-spreading order of tile_tw_slot (stage-twiddle tables,
+// count % 64 == 0 or count < 8 so the permutation stays inside the table).
+SA_HD void ntt_pow_table_thread(fe *out, const fe &base_m, const fe &lead_m, long long count, int swz,
+                                long long thread) {
+    const long long e0 = thread * 16;
+    if (e0 >= count) return;
+    fe acc = fe_montmul(fe_mont_pow_u64(base_m, (uint64_t)e0), lead_m);
+    for (int i = 0; i < 16 && e0 + i < count; i++) {
+        const long long e = e0 + i;
+        tile_st(out + (swz ? (long long)tile_tw_slot((int)e) : e), acc);
+        acc = fe_montmul(acc, base_m);
+    }
+}
+// Thread `idx` of an n1 x n2 matrix: out[k * n2 + j] = w^(k*j) * scale (Montgomery form) for its 16
+// consecutive j; row k is the power table of w^k
+SA_HD void ntt_twb_table_thread(fe *out, const fe &w_m, const fe &scale_m, int n1, int n2, long long idx) {
+    const long long per_row = (n2 + 15) / 16;
+    const long long k = idx / per_row;
+    const long long j0 = (idx % per_row) * 16;
+    if (k >= n1) return;
+    const fe wk = fe_mont_pow_u64(w_m, (uint64_t)k);
+    fe acc = fe_montmul(fe_mont_pow_u64(wk, (uint64_t)j0), scale_m);
+    for (int i = 0; i < 16 && j0 + i < n2; i++) {
+        tile_st(out + k * n2 + j0 + i, acc);
+        acc = fe_montmul(acc, wk);
+    }
+}
 
 struct NttShape {
     int log_n, l1, l2, l3;  // l3 > 0: three passes
@@ -151,6 +184,99 @@ inline void ntt_fill_pass2(TileArgs &a, const fe *tmp, fe *out, const NttShape &
     a.has_scale = 0;
     a.scale = fe_mont_one();
     for (int k = 0; k < 8; k++) a.cst[k] = cst2[k];
+}
+
+// validates the root like ntt.py:10-11: root_m (Montgomery form) must have order exactly n = 2^log_n
+inline int ntt_check_root(const fe &root_m, int log_n) {
+    const uint64_t n = 1ull << log_n;
+    if (!fe_eq(fe_mont_pow_u64(root_m, n), fe_mont_one())) return SA_EROOTORDER;
+    if (fe_eq(fe_mont_pow_u64(root_m, n / 2), fe_mont_one())) return SA_ENOTPRIM;
+    return SA_OK;
+}
+
+// roots of the passes of one transform (Montgomery form)
+struct NttRoots {
+    fe w;           // the transform root: root itself, or root^-1 for intt (ntt.py:29)
+    fe w1, w2, w3;  // roots of the pass-1, pass-2 and pass-3 transforms (one pass: w1 = w)
+    fe wsub;        // three passes: root of the length n2*n3 sub-transforms, base of the pass-2 matrix
+    fe scale;       // n^-1 for intt (ntt.py:27), else 1: in the pass-1 matrix, or applied by a single pass
+};
+inline NttRoots ntt_roots(const NttShape &s, const fe &root_m, int inverse) {
+    NttRoots r;
+    r.w = inverse ? fe_mont_inv(root_m) : root_m;
+    r.scale = inverse ? fe_mont_inv(fe_to_mont(fe_from_u64(1ull << s.log_n))) : fe_mont_one();
+    r.w1 = r.w;
+    r.w2 = r.w3 = r.wsub = fe_mont_one();
+    if (s.l3 > 0) {
+        r.w1 = fe_mont_pow_u64(r.w, 1ull << (s.l2 + s.l3));  // n1-point transforms over j1
+        r.wsub = fe_mont_pow_u64(r.w, 1ull << s.l1);
+        r.w2 = fe_mont_pow_u64(r.wsub, 1ull << s.l3);         // n2-point transforms over j2
+        r.w3 = fe_mont_pow_u64(r.wsub, 1ull << s.l2);         // n3-point transforms over j3
+    } else if (s.l2 > 0) {
+        r.w1 = fe_mont_pow_u64(r.w, 1ull << s.l2);  // root of the length-n1 column transforms
+        r.w2 = fe_mont_pow_u64(r.w, 1ull << s.l1);  // root of the length-n2 row transforms
+    }
+    return r;
+}
+
+// the tables and constants of one transform's passes
+struct NttTables {
+    fe *tw1 = nullptr, *tw2 = nullptr, *tw3 = nullptr;  // stage twiddles of the pass-1, -2, -3 transforms
+    fe *twb = nullptr, *twb2 = nullptr;                 // matrices applied by pass 1 and pass 2
+    fe cst1[8], cst2[8], cst3[8];
+    fe scale_m;  // single pass: n^-1 (Montgomery) for intt
+    int has_scale = 0;
+};
+
+// Builds the tables of a transform of shape s.  pow(&table, base_m, count) makes a stage-twiddle table
+// (ntt_pow_table_thread, lead 1, tile_tw_slot order), twb(&table, w_m, scale_m, rows, cols) a matrix
+// (ntt_twb_table_thread); both return SA_OK or an error code.
+template <class Pow, class Twb>
+int ntt_build_tables(NttTables &t, const NttShape &s, const fe &root_m, int inverse, Pow &&pow, Twb &&twb) {
+    const NttRoots r = ntt_roots(s, root_m, inverse);
+    const int n1 = 1 << s.l1, n2 = 1 << s.l2, n3 = 1 << s.l3;
+    int rc;
+    if ((rc = pow(&t.tw1, r.w1, n1)) != SA_OK) return rc;
+    ntt_fill_cst(t.cst1, r.w1, n1);
+    if (s.l2 == 0) {
+        t.has_scale = inverse ? 1 : 0;
+        t.scale_m = r.scale;
+        return SA_OK;
+    }
+    if ((rc = pow(&t.tw2, r.w2, n2)) != SA_OK) return rc;
+    ntt_fill_cst(t.cst2, r.w2, n2);
+    if (s.l3 == 0) return twb(&t.twb, r.w, r.scale, n1, (long long)n2);
+    if ((rc = pow(&t.tw3, r.w3, n3)) != SA_OK) return rc;
+    ntt_fill_cst(t.cst3, r.w3, n3);
+    if ((rc = twb(&t.twb, r.w, r.scale, n1, (long long)n2 * n3)) != SA_OK) return rc;
+    return twb(&t.twb2, r.wsub, fe_mont_one(), n2, (long long)n3);
+}
+
+// Runs the passes of a transform of shape s: in -> out through tmp (n * batch elements, unused by a single
+// pass; three passes use out as their first intermediate, which is fine when in == out because a tile reads
+// all of its elements before it writes them).  run(logl, a, last) runs one pass of logl-point tile
+// transforms and returns SA_OK or an error code; `last` marks the pass that writes out.
+template <class Run>
+int ntt_run_passes(const NttShape &s, const NttTables &t, const fe *in, fe *out, fe *tmp, size_t batch, Run &&run) {
+    TileArgs a;
+    memset(&a, 0, sizeof(a));
+    int rc;
+    if (s.l2 == 0) {
+        ntt_fill_single(a, in, out, s.log_n, batch, t.tw1, t.cst1, t.has_scale, t.scale_m);
+        return run(s.log_n, a, true);
+    }
+    if (s.l3 > 0) {
+        ntt_fill_3pass_a(a, in, out, s, batch, t.tw1, t.twb, t.cst1);
+        if ((rc = run(s.l1, a, false)) != SA_OK) return rc;
+        ntt_fill_3pass_b(a, out, tmp, s, batch, t.tw2, t.twb2, t.cst2);
+        if ((rc = run(s.l2, a, false)) != SA_OK) return rc;
+        ntt_fill_3pass_c(a, tmp, out, s, batch, t.tw3, t.cst3);
+        return run(s.l3, a, true);
+    }
+    ntt_fill_pass1(a, in, tmp, s, batch, t.tw1, t.twb, t.cst1);
+    if ((rc = run(s.l1, a, false)) != SA_OK) return rc;
+    ntt_fill_pass2(a, tmp, out, s, batch, t.tw2, t.cst2);
+    return run(s.l2, a, true);
 }
 
 }  // namespace sa

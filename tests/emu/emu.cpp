@@ -2,12 +2,16 @@
 // phase functions (stark-anatomy_b200/csrc/*.cuh) on the CPU, thread by thread and
 // barrier phase by barrier phase, so the index maps, twiddle tables and the
 // portable field arithmetic can be checked against the oracle without a GPU.
+// The host-side schedule around them (NTT plan and passes, Merkle launch loop,
+// fold scalars) is the library's own, from the same headers; only the launches
+// are replaced by CPU loops.
 // It is NOT a fallback: nothing in the product loads this library.
 //
 // Build: g++ -O2 -std=c++17 -shared -fPIC -o libsa_emu.so emu.cpp
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
+#include <string>
 #include <vector>
 
 #include "../../stark-anatomy_b200/csrc/field.cuh"
@@ -17,10 +21,6 @@
 #include "../../stark-anatomy_b200/csrc/ntt_tile.cuh"
 
 using namespace sa;
-
-static fe from_limbs(const uint64_t x[2]) {
-    return fe_make((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
-}
 
 static int g_elog = 4, g_c = 8;  // tile shape under test (emu_set_shape)
 
@@ -41,7 +41,7 @@ static void run_tiles_variant(const TileArgs &a) {
     }
 }
 template <int LOGL, int ELOG, int C>
-static void run_tiles(const TileArgs &a) {  // same variant choice as launch_tile (sa_b200.cu)
+static void run_tiles(const TileArgs &a) {  // same variant choice as launch_tile (ntt.cu)
     if constexpr (LOGL >= 5) {
         switch (tile_variant<LOGL, ELOG, C>(a)) {
             case TF_FULL | TF_TWB: return run_tiles_variant<LOGL, ELOG, C, TF_FULL | TF_TWB>(a);
@@ -75,14 +75,16 @@ static void run_tiles_dyn(int logl, const TileArgs &a) {
         case 10: run_tiles_shape<10>(a); break;
     }
 }
-// swz: stage-twiddle tables are stored in tile_tw_slot order (see k_pow_table in sa_b200.cu)
-static std::vector<fe> pow_table(const fe &base_m, const fe &lead_m, size_t count, bool swz = true) {
-    std::vector<fe> t(count);
-    fe acc = lead_m;
-    for (size_t i = 0; i < count; i++) {
-        t[swz ? (size_t)tile_tw_slot((int)i) : i] = acc;
-        acc = fe_montmul(acc, base_m);
-    }
+// the tables of k_pow_table / k_twb_table, thread by thread
+static std::vector<fe> pow_table(const fe &base_m, long long count, int swz) {
+    std::vector<fe> t((size_t)count);
+    for (long long i = 0; i < (count + 15) / 16; i++) ntt_pow_table_thread(t.data(), base_m, fe_mont_one(), count, swz, i);
+    return t;
+}
+static std::vector<fe> twb_table(const fe &w_m, const fe &scale_m, int rows, long long cols) {
+    std::vector<fe> t((size_t)rows * cols);
+    for (long long i = 0; i < rows * ((cols + 15) / 16); i++)
+        ntt_twb_table_thread(t.data(), w_m, scale_m, rows, (int)cols, i);
     return t;
 }
 
@@ -94,41 +96,28 @@ void emu_set_shape(int elog, int c) {
 }
 
 void emu_montmul(uint64_t *out, const uint64_t *a, const uint64_t *b) {
-    fe r = fe_montmul_portable(from_limbs(a), from_limbs(b));
+    fe r = fe_montmul_portable(fe_from_limbs(a), fe_from_limbs(b));
     memcpy(out, &r, 16);
 }
 void emu_mul(uint64_t *out, const uint64_t *a, const uint64_t *b) {
-    fe r = fe_mul(from_limbs(a), from_limbs(b));
+    fe r = fe_mul(fe_from_limbs(a), fe_from_limbs(b));
     memcpy(out, &r, 16);
 }
 void emu_add(uint64_t *out, const uint64_t *a, const uint64_t *b) {
-    fe r = fe_add_portable(from_limbs(a), from_limbs(b));
+    fe r = fe_add_portable(fe_from_limbs(a), fe_from_limbs(b));
     memcpy(out, &r, 16);
 }
 void emu_sub(uint64_t *out, const uint64_t *a, const uint64_t *b) {
-    fe r = fe_sub_portable(from_limbs(a), from_limbs(b));
+    fe r = fe_sub_portable(fe_from_limbs(a), fe_from_limbs(b));
     memcpy(out, &r, 16);
 }
 void emu_inv(uint64_t *out, const uint64_t *a) {
-    fe r = fe_from_mont(fe_mont_inv(fe_to_mont(from_limbs(a))));
+    fe r = fe_from_mont(fe_mont_inv(fe_to_mont(fe_from_limbs(a))));
     memcpy(out, &r, 16);
 }
 
-static std::vector<fe> twb_table(const fe &w_m, const fe &scale_m, size_t rows, size_t cols) {
-    std::vector<fe> t(rows * cols);
-    for (size_t k = 0; k < rows; k++) {
-        const fe wk = fe_mont_pow_u64(w_m, k);
-        fe acc = scale_m;
-        for (size_t j = 0; j < cols; j++) {
-            t[k * cols + j] = acc;
-            acc = fe_montmul(acc, wk);
-        }
-    }
-    return t;
-}
-
-// mirrors sa_ntt (sa_b200.cu): same plan, same tile passes.  force3 != 0 uses the three-pass
-// split (normally only for log_n > 20) so that it can be exercised at small sizes.
+// sa_ntt: the library's plan and pass sequence (ntt_plan.cuh) over the emulated tile passes.  force3 != 0
+// uses the three-pass split (normally only for log_n > 20) so that it can be exercised at small sizes.
 int emu_ntt_ex(uint64_t *out, const uint64_t *in, int log_n, const uint64_t *root, int inverse, size_t batch,
                int force3) {
     const size_t n = size_t(1) << log_n;
@@ -136,57 +125,31 @@ int emu_ntt_ex(uint64_t *out, const uint64_t *in, int log_n, const uint64_t *roo
         memcpy(out, in, 16 * batch);
         return 0;
     }
-    const fe root_m = fe_to_mont(from_limbs(root));
-    if (!fe_eq(fe_mont_pow_u64(root_m, n), fe_mont_one())) return -2;
-    if (fe_eq(fe_mont_pow_u64(root_m, n / 2), fe_mont_one())) return -3;
-    const fe w_m = inverse ? fe_mont_inv(root_m) : root_m;
-    const fe ninv_m = fe_mont_inv(fe_to_mont(fe_from_u64(n)));
-    const fe scale_m = inverse ? ninv_m : fe_mont_one();
+    const fe root_m = fe_to_mont(fe_from_limbs(root));
+    int rc = ntt_check_root(root_m, log_n);
+    if (rc != SA_OK) return rc;
     const NttShape s = ntt_shape(log_n, force3 != 0);
-    TileArgs a;
-    memset(&a, 0, sizeof(a));
-    fe cst1[8], cst2[8], cst3[8];
-    if (s.l3 > 0) {
-        const size_t n1 = size_t(1) << s.l1, n2 = size_t(1) << s.l2, n3 = size_t(1) << s.l3, m = n2 * n3;
-        const fe w1_m = fe_mont_pow_u64(w_m, m);         // n1-point transforms over j1
-        const fe wsub_m = fe_mont_pow_u64(w_m, n1);      // root of the length-m sub-transforms
-        const fe w2_m = fe_mont_pow_u64(wsub_m, n3);     // n2-point transforms over j2
-        const fe w3_m = fe_mont_pow_u64(wsub_m, n2);     // n3-point transforms over j3
-        std::vector<fe> tw1 = pow_table(w1_m, fe_mont_one(), n1), tw2 = pow_table(w2_m, fe_mont_one(), n2),
-                        tw3 = pow_table(w3_m, fe_mont_one(), n3);
-        std::vector<fe> twb1 = twb_table(w_m, scale_m, n1, m), twb2 = twb_table(wsub_m, fe_mont_one(), n2, n3);
-        ntt_fill_cst(cst1, w1_m, (int)n1);
-        ntt_fill_cst(cst2, w2_m, (int)n2);
-        ntt_fill_cst(cst3, w3_m, (int)n3);
-        std::vector<fe> tmp(n * batch);
-        ntt_fill_3pass_a(a, (const fe *)in, (fe *)out, s, batch, tw1.data(), twb1.data(), cst1);
-        run_tiles_dyn(s.l1, a);
-        ntt_fill_3pass_b(a, (const fe *)out, tmp.data(), s, batch, tw2.data(), twb2.data(), cst2);
-        run_tiles_dyn(s.l2, a);
-        ntt_fill_3pass_c(a, tmp.data(), (fe *)out, s, batch, tw3.data(), cst3);
-        run_tiles_dyn(s.l3, a);
-        return 0;
-    }
-    if (log_n <= 10) {
-        std::vector<fe> tw1 = pow_table(w_m, fe_mont_one(), n);
-        ntt_fill_cst(cst1, w_m, (int)n);
-        std::vector<fe> tmp((const fe *)in, (const fe *)in + n * batch);
-        ntt_fill_single(a, tmp.data(), (fe *)out, log_n, batch, tw1.data(), cst1, inverse ? 1 : 0, scale_m);
-        run_tiles_dyn(log_n, a);
-        return 0;
-    }
-    const size_t n1 = size_t(1) << s.l1, n2 = size_t(1) << s.l2;
-    const fe w1_m = fe_mont_pow_u64(w_m, n2), w2_m = fe_mont_pow_u64(w_m, n1);
-    std::vector<fe> tw1 = pow_table(w1_m, fe_mont_one(), n1), tw2 = pow_table(w2_m, fe_mont_one(), n2);
-    std::vector<fe> twb = twb_table(w_m, scale_m, n1, n2);
-    ntt_fill_cst(cst1, w1_m, (int)n1);
-    ntt_fill_cst(cst2, w2_m, (int)n2);
+    std::vector<std::vector<fe>> tables;
+    NttTables t;
+    auto keep = [&](fe **table, std::vector<fe> v) {
+        tables.push_back(std::move(v));
+        *table = tables.back().data();
+        return SA_OK;
+    };
+    ntt_build_tables(
+        t, s, root_m, inverse, [&](fe **table, const fe &base_m, long long count) { return keep(table, pow_table(base_m, count, 1)); },
+        [&](fe **table, const fe &w_m, const fe &scale_m, int rows, long long cols) {
+            return keep(table, twb_table(w_m, scale_m, rows, cols));
+        });
+    // the threads of a tile run one after another here, so a single pass in place would overwrite input
+    // that later threads still read: it reads a copy
     std::vector<fe> tmp(n * batch);
-    ntt_fill_pass1(a, (const fe *)in, tmp.data(), s, batch, tw1.data(), twb.data(), cst1);
-    run_tiles_dyn(s.l1, a);
-    ntt_fill_pass2(a, tmp.data(), (fe *)out, s, batch, tw2.data(), cst2);
-    run_tiles_dyn(s.l2, a);
-    return 0;
+    const fe *src = (const fe *)in;
+    if (s.l2 == 0) src = (const fe *)memcpy(tmp.data(), in, 16 * n * batch);
+    return ntt_run_passes(s, t, src, (fe *)out, tmp.data(), batch, [](int logl, TileArgs &a, bool) {
+        run_tiles_dyn(logl, a);
+        return SA_OK;
+    });
 }
 int emu_ntt(uint64_t *out, const uint64_t *in, int log_n, const uint64_t *root, int inverse, size_t batch) {
     return emu_ntt_ex(out, in, log_n, root, inverse, batch, 0);
@@ -194,13 +157,13 @@ int emu_ntt(uint64_t *out, const uint64_t *in, int log_n, const uint64_t *root, 
 
 uint32_t emu_decimal(uint8_t *buf40, const uint64_t *x) {
     uint64_t w[5];
-    uint32_t n = fe_decimal_words(w, from_limbs(x));
+    uint32_t n = fe_decimal_words(w, fe_from_limbs(x));
     memcpy(buf40, w, 40);
     return n;
 }
 void emu_leaf_digest(uint8_t *out64, const uint64_t *x) {
     uint64_t d[8];
-    merkle_leaf_digest(d, from_limbs(x));
+    merkle_leaf_digest(d, fe_from_limbs(x));
     memcpy(out64, d, 64);
 }
 void emu_node_digest_coop4(uint8_t *out64, const uint8_t *left, const uint8_t *right) {
@@ -218,54 +181,39 @@ void emu_node_digest(uint8_t *out64, const uint8_t *left, const uint8_t *right) 
     memcpy(out64, d, 64);
 }
 
-// mirrors merkle_reduce / k_merkle_chunk (sa_b200.cu): private subtrees, then the shared-memory
-// reduction, heap-ordered tree
-static std::vector<int> g_mk_shape;  // (minlog, ipt_log, chunk_log, red_log, coop_max) rows; tests try other launch shapes
-static void emu_merkle_shape_override(MerkleArgs &a) {
-    int best = -1;
-    const int w = merkle_log2(a.width);
-    for (size_t i = 0; i + 4 < g_mk_shape.size(); i += 5)
-        if (g_mk_shape[i] <= w && g_mk_shape[i] > best && g_mk_shape[i + 2] <= w) {
-            best = g_mk_shape[i];
-            a.ipt_log = g_mk_shape[i + 1];
-            a.chunk = 1 << g_mk_shape[i + 2];
-            a.red_log = g_mk_shape[i + 3];
-            a.coop_max = g_mk_shape[i + 4];
-        }
-}
-static void emu_merkle_reduce(MerkleArgs a) {
+// one launch of k_merkle_chunk without the fused top: private subtrees, then the shared-memory reduction
+static int emu_merkle_chunk(const MerkleArgs &a) {
     std::vector<uint64_t> sm((size_t)MK_THREADS * 8);
-    while (true) {
-        merkle_shape(a);
-        emu_merkle_shape_override(a);
-        const long long blocks = a.width / a.chunk;
-        const int active = a.chunk >> a.ipt_log;
-        for (long long blk = 0; blk < blocks; blk++) {
-            for (int tid = 0; tid < active; tid++) merkle_private(&sm[(size_t)tid * 8], a, blk, tid);
-            long long base = (a.width + blk * a.chunk) >> a.ipt_log;
-            for (int wl = active / 2, lvl = 0; lvl < a.red_log; wl >>= 1, lvl++) {
-                base >>= 1;
-                std::vector<uint64_t> regs((size_t)wl * 8);
-                for (int tid = 0; tid < wl; tid++) {  // phase 1: read children, hash
-                    if (wl > a.coop_max)
-                        merkle_node_digest(&regs[(size_t)tid * 8], &sm[(size_t)(2 * tid) * 8],
-                                           &sm[(size_t)(2 * tid + 1) * 8]);
-                    else  // the four-lanes-per-node schedule of the small levels
-                        blake2b_coop4_node_host(&regs[(size_t)tid * 8], &sm[(size_t)(2 * tid) * 8]);
-                }
-                for (int tid = 0; tid < wl; tid++)  // phase 2: publish
-                    for (int i = 0; i < 8; i++) {
-                        sm[(size_t)tid * 8 + i] = regs[(size_t)tid * 8 + i];
-                        a.tree[(base + tid) * 8 + i] = regs[(size_t)tid * 8 + i];
-                    }
+    const long long blocks = a.width / a.chunk;
+    const int active = a.chunk >> a.ipt_log;
+    for (long long blk = 0; blk < blocks; blk++) {
+        for (int tid = 0; tid < active; tid++) merkle_private(&sm[(size_t)tid * 8], a, blk, tid);
+        long long base = (a.width + blk * a.chunk) >> a.ipt_log;
+        for (int wl = active / 2, lvl = 0; lvl < a.red_log; wl >>= 1, lvl++) {
+            base >>= 1;
+            std::vector<uint64_t> regs((size_t)wl * 8);
+            for (int tid = 0; tid < wl; tid++) {  // phase 1: read children, hash
+                if (wl > a.coop_max)
+                    merkle_node_digest(&regs[(size_t)tid * 8], &sm[(size_t)(2 * tid) * 8],
+                                       &sm[(size_t)(2 * tid + 1) * 8]);
+                else  // the four-lanes-per-node schedule of the small levels
+                    blake2b_coop4_node_host(&regs[(size_t)tid * 8], &sm[(size_t)(2 * tid) * 8]);
             }
+            for (int tid = 0; tid < wl; tid++)  // phase 2: publish
+                for (int i = 0; i < 8; i++) {
+                    sm[(size_t)tid * 8 + i] = regs[(size_t)tid * 8 + i];
+                    a.tree[(base + tid) * 8 + i] = regs[(size_t)tid * 8 + i];
+                }
         }
-        if (merkle_next_width(a) <= 1) break;
-        a.width = merkle_next_width(a);
-        a.mode = 0;
     }
+    return 0;
 }
-void emu_set_merkle_shape(const int *rows, int nrows) { g_mk_shape.assign(rows, rows + 5 * nrows); }
+static std::string g_mk_shape;  // launch shape override in SA_MK_SHAPE form (tests try other launch shapes)
+// the library's launch loop without an arrival counter, which the library falls back to without one
+static void emu_merkle_reduce(const MerkleArgs &a) {
+    merkle_launches(a, nullptr, g_mk_shape.c_str(), [](MerkleArgs &m, bool) { return emu_merkle_chunk(m); });
+}
+void emu_set_merkle_shape(const char *spec) { g_mk_shape = spec ? spec : ""; }
 int emu_merkle_tree(uint8_t *tree, const uint64_t *values, size_t n) {
     memset(tree, 0, 64);
     MerkleArgs a;
@@ -280,8 +228,8 @@ int emu_merkle_tree(uint8_t *tree, const uint64_t *values, size_t n) {
 int emu_fri_round(uint64_t *next, uint8_t *next_tree, const uint64_t *cw, size_t n, const uint64_t *alpha,
                   const uint64_t *offset, const uint64_t *omega) {
     memset(next_tree, 0, 64);
-    const fe winv_m = fe_mont_inv(fe_to_mont(from_limbs(omega)));
-    std::vector<fe> xinv = pow_table(winv_m, fe_mont_one(), n / 2, false);
+    const fe winv_m = fe_mont_inv(fe_to_mont(fe_from_limbs(omega)));
+    std::vector<fe> xinv = pow_table(winv_m, (long long)(n / 2), 0);
     MerkleArgs a;
     memset(&a, 0, sizeof(a));
     a.tree = (uint64_t *)next_tree;
@@ -290,9 +238,7 @@ int emu_fri_round(uint64_t *next, uint8_t *next_tree, const uint64_t *cw, size_t
     a.prev = (const fe *)cw;
     a.next = (fe *)next;
     a.xinv = xinv.data();
-    a.inv2_m = fe_mont_inv(fe_to_mont(fe_from_u64(2)));
-    const fe oinv_m = fe_mont_inv(fe_to_mont(from_limbs(offset)));
-    a.s_m = fe_montmul(fe_montmul(fe_to_mont(from_limbs(alpha)), a.inv2_m), oinv_m);
+    fri_fold_scalars(&a.s_m, &a.inv2_m, fe_from_limbs(alpha), fe_mont_inv(fe_to_mont(fe_from_limbs(offset))));
     emu_merkle_reduce(a);
     return 0;
 }

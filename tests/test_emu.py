@@ -159,10 +159,10 @@ def test_merkle_and_fri_round(E, logn):
 ])
 def test_merkle_other_launch_shapes(E, rows):
     """the generalised launch shape (ipt_log, chunk, red_log) builds the same tree whatever the split"""
-    flat = (ctypes.c_int * (5 * len(rows)))(*[v for r in rows for v in r])
+    spec = ",".join(":".join(str(v) for v in r) for r in rows).encode()  # SA_MK_SHAPE form
     rng = random.Random(77)
     try:
-        E.emu_set_merkle_shape(flat, len(rows))
+        E.emu_set_merkle_shape(spec)
         for logn in (3, 6, 10, 13):
             n = 1 << logn
             x = O.to_np([rng.randrange(P) for _ in range(n)])
@@ -170,4 +170,4 @@ def test_merkle_other_launch_shapes(E, rows):
             E.emu_merkle_tree(O._ptr(tree), O._ptr(x), ctypes.c_size_t(n))
             assert (tree[1:] == O.merkle_tree_np(x)[1:]).all()
     finally:
-        E.emu_set_merkle_shape(flat, 0)
+        E.emu_set_merkle_shape(b"")
