@@ -37,7 +37,6 @@ from merkle import Merkle as _HostMerkle
 from ntt import intt
 
 import sa_engine
-import sa_marshal
 import sa_devlist
 from sa_devlist import DeviceCodeword
 
@@ -73,7 +72,7 @@ class Merkle(_HostMerkle):
         if not isinstance(first, FieldElement) or first.field.p != sa_engine.P:
             return None
         try:
-            packed = sa_marshal.pack(data_array)
+            packed = sa_devlist.pack(data_array)
         except (TypeError, AttributeError, OverflowError):
             return None
         key = blake2b(packed, digest_size=32).digest()
@@ -83,7 +82,7 @@ class Merkle(_HostMerkle):
             return hit[1]
         if hit is not None:  # built by an engine that has since been replaced: its tree is not this engine's
             Merkle._cache_bytes -= 64 * Merkle._trees.pop(key)[1].shape[0]
-        tree = eng.merkle_tree(eng.upload(packed))
+        tree = eng.merkle_tree(sa_devlist.to_device(packed))
         Merkle._trees[key] = (eng, tree)
         Merkle._cache_bytes += 128 * n
         while Merkle._cache_bytes > Merkle._CACHE_LIMIT and len(Merkle._trees) > 1:
@@ -100,13 +99,12 @@ class Merkle(_HostMerkle):
         return sa_engine.get_engine().tree_root(tree)
 
     def open(index, data_array):
-        if isinstance(data_array, DeviceCodeword) and len(data_array) >= 2 and Merkle._device_tree(data_array) is not None:
-            assert(0 <= index and index < len(data_array)), "cannot open invalid index"
-            return data_array.open_paths([index])[0]
         tree = Merkle._device_tree(data_array)
         if tree is None or len(data_array) < 2:
             return _HostMerkle.open(index, list(data_array) if isinstance(data_array, DeviceCodeword) else data_array)
         assert(0 <= index and index < len(data_array)), "cannot open invalid index"
+        if isinstance(data_array, DeviceCodeword):
+            return data_array.open_paths([index])[0]
         return sa_engine.get_engine().merkle_open(tree, [index])[0]
 
 
@@ -178,75 +176,56 @@ class Fri:
         # in HBM: no pack, no upload.
         vecs, trees = eng.fri_commit(sa_devlist.to_device(codeword), rounds, offset, omega, on_root)
 
-        codewords = [codeword]
         if isinstance(codeword, DeviceCodeword):
             codeword.attach_tree(trees[0])
-        else:
-            self._resident[id(codeword)] = (codeword, vecs[0], trees[0])
-        for r in range(1, rounds):
-            codewords.append(DeviceCodeword(vecs[r], trees[r], self.field, N >> r))
+        codewords = [codeword] + [DeviceCodeword(vecs[r], trees[r], self.field, N >> r) for r in range(1, rounds)]
         # send last codeword (a real list: it is pickled into the transcript)
-        last = codewords[-1]
-        if isinstance(last, DeviceCodeword):
-            last = last.tolist()
-            codewords[-1] = last
-        proof_stream.push(last)
-        self._resident[id(last)] = (last, vecs[-1], trees[-1])
+        if isinstance(codewords[-1], DeviceCodeword):
+            codewords[-1] = codewords[-1].tolist()
+        proof_stream.push(codewords[-1])
+        for layer, vec, tree in zip(codewords, vecs, trees):
+            if not isinstance(layer, DeviceCodeword):
+                self._resident[id(layer)] = (layer, vec, tree)
         return codewords
 
     # ---------------------------------------------------------------- query --
-    def _device_layer(self, layer, check=None):
-        """(vector, tree) of a layer: resident from commit, else uploaded and hashed now.
-        check = (indices, elements the caller is about to reveal from a plain list): the reference
-        re-hashes the list it is given on every Merkle.open (merkle.py:26-27), so a list that was
-        modified in place after commit must not be answered from the tree of its old contents; the
-        revealed positions are compared with the resident vector and a mismatch drops the cache."""
+    def _open_layer(self, layer, indices):
+        """(values, authentication paths) of a layer at `indices`.  A DeviceCodeword opens its own tree.  A
+        plain list is opened with one gather from the tree its last commit built, else from a fresh upload
+        and tree: the reference re-hashes the list it is given on every Merkle.open (merkle.py:26-27), so a
+        list that was modified in place after commit must not be answered from the tree of its old contents;
+        the revealed values are compared with the resident vector and a mismatch drops it."""
         if isinstance(layer, DeviceCodeword):
-            return layer.device_vector(), layer.device_tree()
+            layer.prefetch(indices)
+            return [layer[i] for i in indices], layer.open_paths(indices)
         eng = sa_engine.get_engine()
+        values = [layer[i] for i in indices]
         hit = self._resident.get(id(layer))
-        if hit is not None and hit[0] is layer and eng.length(hit[1]) == len(layer):
-            fresh = True
-            if check is not None and len(check[0]):
-                resident = bytes(memoryview(eng.gather(hit[1], list(check[0]))).cast("B"))
-                fresh = resident == bytes(sa_marshal.pack(check[1]))
-            if fresh:
-                return hit[1], hit[2]
-        vec = eng.upload(sa_marshal.pack(layer))
-        tree = eng.merkle_tree(vec)
-        self._resident[id(layer)] = (layer, vec, tree)
-        return vec, tree
+        fresh = hit is not None and hit[0] is layer and eng.length(hit[1]) == len(layer)
+        if fresh and indices:
+            resident = bytes(memoryview(eng.gather(hit[1], indices)).cast("B"))
+            fresh = resident == bytes(sa_devlist.pack(values))
+        if not fresh:
+            vec = sa_devlist.to_device(layer)
+            hit = self._resident[id(layer)] = (layer, vec, eng.merkle_tree(vec))
+        return values, eng.merkle_open(hit[2], indices)
 
     def query(self, current_codeword, next_codeword, c_indices, proof_stream):
-        eng = sa_engine.get_engine()
         # infer a and b indices
         a_indices = [index for index in c_indices]
         b_indices = [index + len(current_codeword) // 2 for index in c_indices]
-        s_range = range(self.num_colinearity_tests)
+        k = self.num_colinearity_tests
+        s_range = range(k)
         ab = [a_indices[s] for s in s_range] + [b_indices[s] for s in s_range]
         cc = [c_indices[s] for s in s_range]
-
-        if isinstance(current_codeword, DeviceCodeword):
-            current_codeword.prefetch(ab)
-        if isinstance(next_codeword, DeviceCodeword):
-            next_codeword.prefetch(cc)
+        cur, cur_paths = self._open_layer(current_codeword, ab)
+        nxt, nxt_paths = self._open_layer(next_codeword, cc)
 
         # reveal leafs
         for s in s_range:
-            proof_stream.push((current_codeword[a_indices[s]], current_codeword[b_indices[s]], next_codeword[c_indices[s]]))
+            proof_stream.push((cur[s], cur[k + s], nxt[s]))
 
-        # reveal authentication paths: one gather per layer from the resident trees
-        if isinstance(current_codeword, DeviceCodeword):
-            cur_paths = current_codeword.open_paths(ab)
-        else:
-            _, cur_tree = self._device_layer(current_codeword, (ab, [current_codeword[i] for i in ab]))
-            cur_paths = eng.merkle_open(cur_tree, ab)
-        if isinstance(next_codeword, DeviceCodeword):
-            nxt_paths = next_codeword.open_paths(cc)
-        else:
-            _, nxt_tree = self._device_layer(next_codeword, (cc, [next_codeword[i] for i in cc]))
-            nxt_paths = eng.merkle_open(nxt_tree, cc)
-        k = self.num_colinearity_tests
+        # reveal authentication paths
         for s in s_range:
             proof_stream.push(cur_paths[s])
             proof_stream.push(cur_paths[k + s])

@@ -22,10 +22,8 @@ fast_coset_evaluate :132-135, fast_coset_divide :137-176.
 import sa_host  # noqa: F401  (resolves algebra/univariate: the reference's, else the host mirror)
 from univariate import *  # noqa: F401,F403  re-exported exactly like code/ntt.py:1
 from univariate import Polynomial
-from algebra import FieldElement
 
 import sa_engine
-import sa_marshal
 import sa_devlist
 import sa_accel  # noqa: F401  (opt-in Polynomial.__mul__ acceleration; inert unless enabled)
 
@@ -53,18 +51,6 @@ def _check_root(primitive_root, root_order):
 
 def _log2(n):
     return n.bit_length() - 1
-
-
-def _unpack(vec_or_buf, field):
-    eng = _engine()
-    buf = vec_or_buf if isinstance(vec_or_buf, (bytes, bytearray, memoryview)) else eng.download(vec_or_buf)
-    return sa_marshal.unpack(buf, field, FieldElement)
-
-
-def _upload_padded(elements, total):
-    """pack `elements`, upload, zero-pad on the device to `total` elements"""
-    eng = _engine()
-    return eng.pad(eng.upload(sa_marshal.pack(elements)), total)
 
 
 # --------------------------------------------------------------------- ntt --
@@ -110,6 +96,21 @@ def _transform_length(ncoef, order):
     return total
 
 
+def _ntt_product(a, b, root, pointwise):
+    """ntt.py:52-64 on two zero-padded coefficient vectors: transform both, combine the codewords with
+    `pointwise` (eng.pointwise_mul / eng.pointwise_div), transform back"""
+    eng = _engine()
+    ln, rn = eng.length(a), eng.length(b)
+    a = eng.ntt(a, _log2(ln), root)
+    b = eng.ntt(b, _log2(rn), root)
+    if ln != rn:  # the reference's zip() truncates to the shorter codeword (ntt.py:61)
+        k = min(ln, rn)
+        a, b = eng.slice(a, 0, k), eng.slice(b, 0, k)
+        assert(k & (k - 1) == 0), "cannot compute intt of non-power-of-two sequence"
+    combined = pointwise(a, b)
+    return eng.ntt(combined, _log2(eng.length(combined)), root, inverse=True)
+
+
 def fast_multiply(lhs, rhs, primitive_root, root_order):
     _check_root(primitive_root, root_order)
     if lhs.is_zero() or rhs.is_zero():
@@ -124,15 +125,10 @@ def fast_multiply(lhs, rhs, primitive_root, root_order):
     eng = _engine()
     ln = _transform_length(lhs_degree + 1, order)
     rn = _transform_length(rhs_degree + 1, order)
-    a = eng.ntt(_upload_padded(lhs.coefficients[:lhs_degree + 1], ln), _log2(ln), root)
-    b = eng.ntt(_upload_padded(rhs.coefficients[:rhs_degree + 1], rn), _log2(rn), root)
-    if ln != rn:  # the reference's zip() truncates to the shorter codeword (ntt.py:61)
-        k = min(ln, rn)
-        a, b = eng.slice(a, 0, k), eng.slice(b, 0, k)
-        assert(k & (k - 1) == 0), "cannot compute intt of non-power-of-two sequence"
-    hadamard = eng.pointwise_mul(a, b)
-    product = eng.ntt(hadamard, _log2(eng.length(hadamard)), root, inverse=True)
-    return Polynomial(_unpack(eng.slice(product, 0, degree + 1), field))
+    a = eng.pad(sa_devlist.to_device(lhs.coefficients[:lhs_degree + 1]), ln)
+    b = eng.pad(sa_devlist.to_device(rhs.coefficients[:rhs_degree + 1]), rn)
+    product = _ntt_product(a, b, root, eng.pointwise_mul)
+    return Polynomial(sa_devlist.from_device(eng.slice(product, 0, degree + 1), field))
 
 
 def fast_zerofier(domain, primitive_root, root_order):
@@ -147,7 +143,7 @@ def fast_zerofier(domain, primitive_root, root_order):
         # prod (X - d): the subproduct tree of ntt.py:76-80 yields this same monic polynomial,
         # len(domain) + 1 coefficients; one device kernel builds it
         _check_field(field)
-        return Polynomial(_unpack(eng.zerofier(eng.upload(sa_marshal.pack(domain))), field))
+        return Polynomial(sa_devlist.from_device(eng.zerofier(sa_devlist.to_device(domain)), field))
     half = len(domain) // 2
     left = fast_zerofier(domain[:half], primitive_root, root_order)
     right = fast_zerofier(domain[half:], primitive_root, root_order)
@@ -165,9 +161,8 @@ def fast_evaluate(polynomial, domain, primitive_root, root_order):
     # the remainder tree of the reference (ntt.py:94-100) only re-expresses
     # polynomial(d) for every d in the domain; one Horner kernel gives the same values
     eng = _engine()
-    values = eng.poly_eval(eng.upload(sa_marshal.pack(polynomial.coefficients)),
-                           eng.upload(sa_marshal.pack(domain)))
-    return _unpack(values, field)
+    values = eng.poly_eval(sa_devlist.to_device(polynomial.coefficients), sa_devlist.to_device(domain))
+    return sa_devlist.from_device(values, field)
 
 
 def fast_interpolate(domain, values, primitive_root, root_order):
@@ -184,8 +179,8 @@ def fast_interpolate(domain, values, primitive_root, root_order):
         # coinciding domain points raise "divide by zero" like the division at ntt.py:124-125
         field = values[0].field
         _check_field(field)
-        coeffs = eng.interpolate(eng.upload(sa_marshal.pack(domain)), eng.upload(sa_marshal.pack(values)))
-        return Polynomial(_unpack(coeffs, field))
+        coeffs = eng.interpolate(sa_devlist.to_device(domain), sa_devlist.to_device(values))
+        return Polynomial(sa_devlist.from_device(coeffs, field))
     half = len(domain) // 2
     left_zerofier = fast_zerofier(domain[:half], primitive_root, root_order)
     right_zerofier = fast_zerofier(domain[half:], primitive_root, root_order)
@@ -209,7 +204,7 @@ def fast_coset_evaluate(polynomial, offset, generator, order):
     eng = _engine()
     if total <= 1:
         return polynomial.scale(offset).coefficients + [field.zero()] * (order - ncoef)
-    coeffs = eng.upload(sa_marshal.pack(polynomial.coefficients))
+    coeffs = sa_devlist.to_device(polynomial.coefficients)
     scaled = eng.pad(eng.scale(coeffs, offset.value), total) if ncoef else eng.zeros(total)
     return sa_devlist.wrap(eng.ntt(scaled, _log2(total), generator.value), field)
 
@@ -231,15 +226,8 @@ def fast_coset_divide(lhs, rhs, offset, primitive_root, root_order):  # clean di
     ln = _transform_length(lhs_degree + 1, order)
     rn = _transform_length(rhs_degree + 1, order)
     # scale(offset) then trim to degree+1 (ntt.py:159-166) == scale the trimmed coefficients
-    a = eng.pad(eng.scale(eng.upload(sa_marshal.pack(lhs.coefficients[:lhs_degree + 1])), offset.value), ln)
-    b = eng.pad(eng.scale(eng.upload(sa_marshal.pack(rhs.coefficients[:rhs_degree + 1])), offset.value), rn)
-    a = eng.ntt(a, _log2(ln), root)
-    b = eng.ntt(b, _log2(rn), root)
-    if ln != rn:
-        k = min(ln, rn)
-        a, b = eng.slice(a, 0, k), eng.slice(b, 0, k)
-        assert(k & (k - 1) == 0), "cannot compute intt of non-power-of-two sequence"
-    quotient_codeword = eng.pointwise_div(a, b)  # raises "divide by zero" like algebra.py:92
-    scaled_quotient = eng.ntt(quotient_codeword, _log2(eng.length(quotient_codeword)), root, inverse=True)
+    a = eng.pad(eng.scale(sa_devlist.to_device(lhs.coefficients[:lhs_degree + 1]), offset.value), ln)
+    b = eng.pad(eng.scale(sa_devlist.to_device(rhs.coefficients[:rhs_degree + 1]), offset.value), rn)
+    scaled_quotient = _ntt_product(a, b, root, eng.pointwise_div)  # raises "divide by zero" like algebra.py:92
     kept = eng.slice(scaled_quotient, 0, lhs_degree - rhs_degree + 1)
-    return Polynomial(_unpack(eng.scale(kept, offset.inverse().value), field))
+    return Polynomial(sa_devlist.from_device(eng.scale(kept, offset.inverse().value), field))

@@ -18,10 +18,10 @@ import os
 
 import sa_host
 import sa_engine
-import sa_marshal
+import sa_devlist
+import ntt  # the drop-in, which imports this module in turn; device_mul only runs once both are loaded
 
 Polynomial = sa_host.univariate.Polynomial
-FieldElement = sa_host.algebra.FieldElement
 
 _original_mul = None
 THRESHOLD = 2048  # len(a) * len(b) below this stays on the host loop
@@ -39,15 +39,11 @@ def device_mul(self, other):
     if len(a) * len(b) < THRESHOLD or a[0].field.p != sa_engine.P:
         return _original_mul(self, other)
     out_len = len(a) + len(b) - 1
-    log_n = max((out_len - 1).bit_length(), 1)
-    n = 1 << log_n
+    n = 1 << max((out_len - 1).bit_length(), 1)
     eng = sa_engine.get_engine()
-    w = _root_of_unity(n)
-    fa = eng.ntt(eng.pad(eng.upload(sa_marshal.pack(a)), n), log_n, w)
-    fb = eng.ntt(eng.pad(eng.upload(sa_marshal.pack(b)), n), log_n, w)
-    prod = eng.ntt(eng.pointwise_mul(fa, fb), log_n, w, inverse=True)
-    coeffs = sa_marshal.unpack(eng.download(eng.slice(prod, 0, out_len)), a[0].field, FieldElement)
-    return Polynomial(coeffs)
+    fa, fb = eng.pad(sa_devlist.to_device(a), n), eng.pad(sa_devlist.to_device(b), n)
+    prod = ntt._ntt_product(fa, fb, _root_of_unity(n), eng.pointwise_mul)
+    return Polynomial(sa_devlist.from_device(eng.slice(prod, 0, out_len), a[0].field))
 
 
 def enable(threshold=None):

@@ -20,6 +20,9 @@ List semantics that the reference's callers rely on are kept:
 ``tolist()`` gives the real list (materialised once, identities handed out earlier are kept);
 pickling a DeviceCodeword pickles that list.  SA_B200_DEVICE_LISTS=0 makes the drop-in return plain lists
 everywhere (the round-1 behaviour).
+
+``to_device`` / ``from_device`` at the end of this module are the drop-in's only conversions between a
+sequence of field elements and an engine vector.
 """
 import os
 
@@ -52,8 +55,7 @@ class DeviceCodeword:
     def device_vector(self):
         """the values as an engine vector; re-packed and re-uploaded only after a mutation"""
         if self._dirty:
-            eng = sa_engine.get_engine()
-            self._vec = eng.upload(sa_marshal.pack(self._full))
+            self._vec = to_device(self._full)
             self._len = len(self._full)
             self._dirty = False
         return self._vec
@@ -81,7 +83,7 @@ class DeviceCodeword:
         # one index at a time (code/fast_stark.py:162-174 opens 1024 positions one by one): fetch a small tree once
         # and read the paths on the host; a batch of indices (Fri.query) is one gather on the device
         indices = list(indices)
-        if n <= SMALL_TREE and hasattr(eng, "download_tree") and (self._host_tree is not None or len(indices) <= 2):
+        if n <= SMALL_TREE and (self._host_tree is not None or len(indices) <= 2):
             if self._host_tree is None:
                 self._host_tree = eng.download_tree(tree)
             host, depth = self._host_tree, n.bit_length() - 1
@@ -113,7 +115,7 @@ class DeviceCodeword:
 
     def tolist(self):
         if self._full is None:
-            full = sa_marshal.unpack(sa_engine.get_engine().download(self._vec), self._field, FieldElement)
+            full = from_device(self._vec, self._field)
             for i, el in self._cache.items():  # keep identities handed out earlier
                 full[i] = el
             self._full = full
@@ -238,15 +240,26 @@ def wrap(vec, field, tree=None):
     """what ntt / intt / fast_coset_evaluate return: the device list, or a real list when disabled"""
     if ENABLED:
         return DeviceCodeword(vec, tree, field)
-    return sa_marshal.unpack(sa_engine.get_engine().download(vec), field, FieldElement)
+    return from_device(vec, field)
+
+
+def pack(seq):
+    """the host form of a sequence of field elements, 16 little-endian bytes per residue: what
+    ``to_device`` uploads, and what fri.py fingerprints and compares revealed values in"""
+    return sa_marshal.pack(seq)
 
 
 def to_device(seq):
     """engine vector of a sequence of field elements: the resident vector of a DeviceCodeword, else
-    pack + upload"""
+    pack + upload (the bytearray ``pack`` returns is uploaded as it is)"""
     if isinstance(seq, DeviceCodeword):
         return seq.device_vector()
-    return sa_engine.get_engine().upload(sa_marshal.pack(seq))
+    return sa_engine.get_engine().upload(seq if isinstance(seq, bytearray) else sa_marshal.pack(seq))
+
+
+def from_device(vec, field):
+    """list of ``FieldElement`` of `field` holding the values of an engine vector: download + unpack"""
+    return sa_marshal.unpack(sa_engine.get_engine().download(vec), field, FieldElement)
 
 
 def field_of(seq):
