@@ -42,7 +42,7 @@ enum {
     SA_ENOTPRIM = -3,   /* ntt.py:11  "primitive root is not primitive nth root of unity, ..." */
     SA_EDIVZERO = -4,   /* algebra.py:92 "divide by zero" (element-wise division, ntt.py:172) */
     SA_EINDEX = -5,     /* merkle.py:18 "cannot open invalid index" */
-    SA_ESIZE = -6,      /* unsupported size (log_n > 26, n == 0, ...) */
+    SA_ESIZE = -6,      /* unsupported size (log_n > 30, n == 0, ...) */
     SA_ECALLBACK = -7,  /* the challenge callback of sa_fri_commit returned non-zero */
     SA_ECUDA = -100     /* CUDA runtime error; sa_last_error() has the text */
 };
@@ -59,7 +59,9 @@ uint64_t sa_launch_count(void);
  * contiguous transforms of n = 2^log_n elements.  inverse != 0 computes intt: the
  * transform with root^-1 followed by the multiplication with n^-1.
  * Validates root^n == 1 and root^(n/2) != 1 exactly like the reference's asserts.
- * in == out is allowed.  log_n in [0, 26].                                               */
+ * in == out is allowed.  log_n in [0, 30]; a transform of n elements needs a workspace of n
+ * elements besides its input and output (16 GiB each at 2^30).  The caller's buffers must hold
+ * batch * n elements: the library cannot check their length.                              */
 int sa_ntt(void *out, const void *in, int log_n, const uint64_t root[2], int inverse, size_t batch,
            void *stream);
 /* Multi-GPU assembly (SURVEY 8e; no reference counterpart: the reference is one thread on one CPU).

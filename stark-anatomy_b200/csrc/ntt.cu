@@ -160,6 +160,15 @@ static int launch_tile_variant(const TileArgs &a, cudaStream_t st) {
 template <int LOGL, int ELOG, int C>
 static int launch_tile(const TileArgs &a, cudaStream_t st) {
     const int variant = tile_variant<LOGL, ELOG, C>(a);
+    if (variant & TF_TWB2) {
+        // factored pass-1 twiddles exist only above 2^26, where pass 1 runs 2^9- or 2^10-point tiles in the
+        // shape launch_tile_shape gives a pass without peers (tuning shapes of -DSA_TUNE do not have them)
+        if constexpr (LOGL >= 9 && ELOG == 4 && C == 4) {
+            if (variant & TF_FULL) return launch_tile_variant<LOGL, ELOG, C, TF_FULL | TF_TWB2>(a, st);
+            return launch_tile_variant<LOGL, ELOG, C, TF_DYNAMIC | TF_TWB2>(a, st);
+        }
+        return SA_ESIZE;
+    }
     if constexpr (LOGL >= 5) {
         switch (variant) {
             case TF_FULL | TF_TWB: return launch_tile_variant<LOGL, ELOG, C, TF_FULL | TF_TWB>(a, st);
@@ -328,6 +337,20 @@ int sa_ntt_host(void *out_host, const void *in_host, int log_n, const uint64_t r
     const size_t bytes = one * batch;
     if (bytes == 0) return SA_OK;
     int rc;
+    if (log_n > NTT_FULL_TWB_MAX_LOG_N) {
+        // a transform above 2^26 is a chunk of its own, and every pipelined chunk would hold a staging buffer
+        // and an n-element intermediate per copy stream (32 GiB at 2^28): one transform at a time instead,
+        // through one staging buffer on `st`
+        void *dev = nullptr;
+        if ((rc = get_workspace(&dev, one, st, 1)) != SA_OK) return rc;
+        for (size_t b = 0; b < batch && rc == SA_OK; b++) {
+            SA_CUDA(cudaMemcpyAsync(dev, (const char *)in_host + b * one, one, cudaMemcpyHostToDevice, st));
+            rc = sa_ntt(dev, dev, log_n, root, inverse, 1, stream);
+            if (rc == SA_OK) SA_CUDA(cudaMemcpyAsync((char *)out_host + b * one, dev, one, cudaMemcpyDeviceToHost, st));
+        }
+        SA_CUDA(cudaStreamSynchronize(st));
+        return rc;
+    }
     CopySet *cset = nullptr;
     if ((rc = get_copy_set(&cset)) != SA_OK) return rc;
     // chunk = as many transforms as fit g_host_chunk (default two 2^20 transforms); small jobs stay on `st`

@@ -14,6 +14,9 @@
 //       pass 1: n1-point transforms over j1 (stride n2 n3), times w^(k1*m), m = j2*n3 + j3;
 //       pass 2: inside every k1 block, n2-point transforms over j2 (stride n3), times (w^n1)^(k2*j3);
 //       pass 3: n3-point transforms over j3 (contiguous), written to out[k1 + n1*k2 + n1*n2*k3].
+//   log_n 27..30: the same three passes, but the pass-1 matrix w^(k1*m) would have n entries (16 GiB at
+//       2^30).  With m = j2*n3 + j3 it factors as (w^n3)^(k1*j2) * w^(k1*j3): pass 1 multiplies by one entry
+//       of an n1 x n2 table A (which also carries n^-1 for intt) and one of an n1 x n3 table B.
 #pragma once
 #include <cstring>
 
@@ -22,7 +25,10 @@
 
 namespace sa {
 
-constexpr int NTT_MAX_LOG_N = 26;  // the pass-1 twiddle matrix has n entries (1 GiB at 2^26)
+// every digit of the three-pass split stays <= 10 (one tile) and every in-tile row offset below 2^31
+constexpr int NTT_MAX_LOG_N = 30;
+// largest size whose pass-1 twiddles are one n-entry matrix (1 GiB at 2^26); above it they are factored
+constexpr int NTT_FULL_TWB_MAX_LOG_N = 26;
 
 // Thread `thread` of a power table: out[slot(e)] = base^e * lead (Montgomery form) for its 16 consecutive
 // exponents e < count.  swz != 0 stores in the bank-spreading order of tile_tw_slot (stage-twiddle tables,
@@ -55,12 +61,15 @@ SA_HD void ntt_twb_table_thread(fe *out, const fe &w_m, const fe &scale_m, int n
 
 struct NttShape {
     int log_n, l1, l2, l3;  // l3 > 0: three passes
+    int twb_split;          // three passes with the pass-1 matrix factored into A (n1 x n2) and B (n1 x n3)
 };
-// force3: split into three digits even when two would do (tests exercise the 3-pass path small)
-SA_HD NttShape ntt_shape(int log_n, bool force3 = false) {
+// force3: 1 = split into three digits even when two would do, 2 = the same with factored pass-1 twiddles
+// (tests exercise both three-pass plans at small sizes); 0 = the plan of the size
+SA_HD NttShape ntt_shape(int log_n, int force3 = 0) {
     NttShape s;
     s.log_n = log_n;
     s.l3 = 0;
+    s.twb_split = 0;
     if (log_n <= 10 && !force3) {
         s.l1 = log_n;
         s.l2 = 0;
@@ -71,6 +80,7 @@ SA_HD NttShape ntt_shape(int log_n, bool force3 = false) {
         s.l3 = log_n / 3;
         s.l1 = (log_n + 2) / 3;
         s.l2 = log_n - s.l1 - s.l3;
+        s.twb_split = s.l3 > 0 && (log_n > NTT_FULL_TWB_MAX_LOG_N || force3 == 2) ? 1 : 0;
     }
     return s;
 }
@@ -96,15 +106,21 @@ inline void ntt_fill_common(TileArgs &a) {
     a.twb_stride = 0;
     a.npeer = 0;
     a.mc_out = nullptr;
+    a.twb_b = nullptr;
 }
 // three-pass split (see the header comment).  tmp: n * batch workspace; out doubles as the first
 // intermediate (a tile reads all of its elements before it writes them, so in == out is fine).
+// twb1_b != nullptr: factored pass-1 twiddles, twb1 = A (n1 x n2) and twb1_b = B (n1 x n3)
 inline void ntt_fill_3pass_a(TileArgs &a, const fe *in, fe *mid, const NttShape &s, size_t batch, const fe *tw1,
-                             const fe *twb1, const fe cst1[8]) {
+                             const fe *twb1, const fe *twb1_b, const fe cst1[8]) {
     const long long n = 1ll << s.log_n, m = 1ll << (s.l2 + s.l3);
     ntt_fill_common(a);
     a.in = in; a.out = mid; a.tw = tw1;
     a.twb = twb1; a.twb_stride = m;
+    if (twb1_b != nullptr) {  // columns m = j2 * n3 + j3: A has n2 columns, B the remaining n3 = m / n2
+        a.twb_stride = 1ll << s.l2;
+        a.twb_b = twb1_b;
+    }
     a.in_sr = m; a.in_sc = 1; a.in_sb = n;
     a.out_sr = m; a.out_sc = 1; a.out_sb = n;
     a.ncols = (int)m; a.nbatch = (int)batch;
@@ -223,6 +239,7 @@ inline NttRoots ntt_roots(const NttShape &s, const fe &root_m, int inverse) {
 struct NttTables {
     fe *tw1 = nullptr, *tw2 = nullptr, *tw3 = nullptr;  // stage twiddles of the pass-1, -2, -3 transforms
     fe *twb = nullptr, *twb2 = nullptr;                 // matrices applied by pass 1 and pass 2
+    fe *twb_b = nullptr;  // factored pass-1 twiddles (twb_split): twb = A, twb_b = B
     fe cst1[8], cst2[8], cst3[8];
     fe scale_m;  // single pass: n^-1 (Montgomery) for intt
     int has_scale = 0;
@@ -248,7 +265,13 @@ int ntt_build_tables(NttTables &t, const NttShape &s, const fe &root_m, int inve
     if (s.l3 == 0) return twb(&t.twb, r.w, r.scale, n1, (long long)n2);
     if ((rc = pow(&t.tw3, r.w3, n3)) != SA_OK) return rc;
     ntt_fill_cst(t.cst3, r.w3, n3);
-    if ((rc = twb(&t.twb, r.w, r.scale, n1, (long long)n2 * n3)) != SA_OK) return rc;
+    if (s.twb_split) {
+        // A[k1][j2] = (w^n3)^(k1*j2) * scale, B[k1][j3] = w^(k1*j3): A * B = w^(k1*(j2*n3 + j3)) * scale
+        if ((rc = twb(&t.twb, fe_mont_pow_u64(r.w, (uint64_t)n3), r.scale, n1, (long long)n2)) != SA_OK) return rc;
+        if ((rc = twb(&t.twb_b, r.w, fe_mont_one(), n1, (long long)n3)) != SA_OK) return rc;
+    } else if ((rc = twb(&t.twb, r.w, r.scale, n1, (long long)n2 * n3)) != SA_OK) {
+        return rc;
+    }
     return twb(&t.twb2, r.wsub, fe_mont_one(), n2, (long long)n3);
 }
 
@@ -266,7 +289,7 @@ int ntt_run_passes(const NttShape &s, const NttTables &t, const fe *in, fe *out,
         return run(s.log_n, a, true);
     }
     if (s.l3 > 0) {
-        ntt_fill_3pass_a(a, in, out, s, batch, t.tw1, t.twb, t.cst1);
+        ntt_fill_3pass_a(a, in, out, s, batch, t.tw1, t.twb, t.twb_b, t.cst1);
         if ((rc = run(s.l1, a, false)) != SA_OK) return rc;
         ntt_fill_3pass_b(a, out, tmp, s, batch, t.tw2, t.twb2, t.cst2);
         if ((rc = run(s.l2, a, false)) != SA_OK) return rc;

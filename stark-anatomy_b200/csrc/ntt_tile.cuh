@@ -56,11 +56,17 @@ struct TileArgs {
     // ... or ONE multicast address (NVLink SHARP / NVLS: a multicast object with every rank's buffer bound to it):
     // a single multimem.st leaves the GPU and the switch delivers it to every rank's buffer, the own one included
     fe *mc_out;
+    // factored output twiddle (TF_TWB2 kernels only): the ncols = n2 * n3 columns split as col = j2 * n3 + j3
+    // with n2 = twb_stride, and the factor of row k is twb[k * n2 + j2] * twb_b[k * n3 + j3].  (One pointer
+    // fills the struct's tail padding, so the kernel parameters after it keep their offsets.)
+    const fe *twb_b;
 };
+static_assert(sizeof(TileArgs) == 352, "TileArgs outgrew its tail padding: every tile kernel's parameters move");
 
 // kernel variants: with TF_DYNAMIC everything is decided at run time (partial tiles, optional
-// output twiddle / scale); the static variants drop the predication and branches
-enum { TF_FULL = 1, TF_TWB = 2, TF_SCALE = 4, TF_DYNAMIC = 8, TF_PEERS = 16 };
+// output twiddle / scale); the static variants drop the predication and branches.  TF_TWB2 applies the
+// factored output twiddle (twb and twb_b), in full-tile or dynamic kernels; it is never decided at run time.
+enum { TF_FULL = 1, TF_TWB = 2, TF_SCALE = 4, TF_DYNAMIC = 8, TF_PEERS = 16, TF_TWB2 = 32 };
 
 template <int LOGL, int ELOG, int C>
 struct TilePlan {
@@ -88,6 +94,15 @@ struct TilePlan {
 // strided look-ups of the middle stages ((k*m) << 3: all multiples of 8) spread over the eight
 // 16-byte bank groups of shared memory instead of piling onto one
 SA_HDC int tile_tw_slot(int e) { return e ^ ((e >> 3) & 7); }
+
+// log2 of a power of two
+SA_HD int tile_log2(unsigned x) {
+#if defined(__CUDA_ARCH__)
+    return __ffs(x) - 1;
+#else
+    return __builtin_ctz(x);
+#endif
+}
 
 SA_HDC int tile_bitrev(int i, int r) {
     int j = 0;
@@ -285,10 +300,19 @@ SA_HD void ntt_tile_last_stage(int t, fe *sm, const TileArgs &a, long long b, in
     const int c = t % C, q = t / C;
     const int col = col0 + c;
     const bool active = (FLAGS & TF_FULL) ? true : (valid && col < a.ncols);
+    constexpr bool TWB2 = (FLAGS & TF_TWB2) != 0;
     const bool use_twb = (FLAGS & TF_DYNAMIC) ? (a.twb != nullptr) : ((FLAGS & TF_TWB) != 0);
     const bool use_scale = (FLAGS & TF_DYNAMIC) ? (a.has_scale != 0) : ((FLAGS & TF_SCALE) != 0);
     const fe *twb = use_twb ? a.twb + col : nullptr;
     const unsigned out_sr = (unsigned)a.out_sr, twb_sr = (unsigned)a.twb_stride;
+    // factored twiddle: the row-k factor is twb_a[k * twb_sr] * twb_b[k * twb_b_sr]
+    const fe *twb_a = nullptr, *twb_b = nullptr;
+    unsigned twb_b_sr = 0;
+    if constexpr (TWB2) {
+        twb_b_sr = (unsigned)a.ncols / twb_sr;  // n3, a power of two
+        twb_a = a.twb + ((unsigned)col >> tile_log2(twb_b_sr));
+        twb_b = a.twb_b + ((unsigned)col & (twb_b_sr - 1));
+    }
     fe *dst = a.out + tile_batch_offset(b, a.inner, a.out_sb, a.out_sb2) + (long long)col * a.out_sc;
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
@@ -315,7 +339,11 @@ SA_HD void ntt_tile_last_stage(int t, fe *sm, const TileArgs &a, long long b, in
         for (int k = 0; k < R; k++) {
             const unsigned o = (unsigned)tile_digit_reverse<LOGL, ELOG, C>(row0 + k);
             fe v = x[k];
-            if (use_twb && active) v = fe_montmul(v, tile_ldg(twb + o * twb_sr));
+            if constexpr (TWB2) {
+                if (active) v = fe_montmul(fe_montmul(v, tile_ldg(twb_a + o * twb_sr)), tile_ldg(twb_b + o * twb_b_sr));
+            } else if (use_twb && active) {
+                v = fe_montmul(v, tile_ldg(twb + o * twb_sr));
+            }
             if (use_scale) v = fe_montmul(v, a.scale);
             if (active) {
                 if constexpr ((FLAGS & TF_PEERS) != 0) {
@@ -356,6 +384,10 @@ SA_HD int tile_variant(const TileArgs &a) {
     using P = TilePlan<LOGL, ELOG, C>;
     const long long tiles = (long long)((a.ncols + C - 1) / C) * a.nbatch;
     const int peers = (a.npeer > 0 || a.mc_out != nullptr) ? TF_PEERS : 0;
+    if (a.twb_b != nullptr) {  // factored output twiddle: pass 1 of a three-pass plan, so no peers
+        const bool full = LOGL >= 5 && a.ncols % C == 0 && tiles % P::TPC == 0 && !a.has_scale;
+        return TF_TWB2 | (full ? TF_FULL : TF_DYNAMIC);
+    }
     if (LOGL < 5 || a.ncols % C != 0 || tiles % P::TPC != 0 || a.has_scale) return TF_DYNAMIC | peers;
     if (peers) return a.twb == nullptr ? (TF_FULL | TF_PEERS) : (TF_DYNAMIC | TF_PEERS);
     return TF_FULL | (a.twb != nullptr ? TF_TWB : 0);

@@ -173,7 +173,15 @@ class CudaEngine:
         return self.torch.cat(vecs, dim=0)
 
     # ------------------------------------------------------------------ ntt
+    @staticmethod
+    def _check_ntt_length(vec, log_n, batch):
+        """the library reads batch << log_n elements of the input: a shorter vector is refused here, before any
+        device work (the library cannot see a buffer's length)"""
+        if log_n >= 0 and vec.shape[0] < batch << log_n:
+            raise SaError(SA_ERRORS[-6])
+
     def ntt(self, vec, log_n, root, inverse=False, batch=1):
+        self._check_ntt_length(vec, log_n, batch)
         vec = vec.contiguous()
         out = self.empty(vec.shape[0])
         self._check(self.lib.sa_ntt(out.data_ptr(), vec.data_ptr(), log_n, _limbs(root), int(bool(inverse)),
@@ -183,6 +191,7 @@ class CudaEngine:
     def ntt_into(self, out, vec, log_n, root, inverse=False, batch=1):
         """sa_ntt into a caller-provided device vector (a slice of a larger buffer); out may alias vec"""
         assert out.is_contiguous() and vec.is_contiguous() and out.shape[0] == vec.shape[0]
+        self._check_ntt_length(vec, log_n, batch)
         self._check(self.lib.sa_ntt(out.data_ptr(), vec.data_ptr(), log_n, _limbs(root), int(bool(inverse)), batch,
                                     self._stream()))
         return out
@@ -190,6 +199,7 @@ class CudaEngine:
     def ntt_multi(self, outs, out_offset, vec, log_n, root, inverse=False, batch=1):
         """sa_ntt_multi: transform `vec` and store the result at element offset `out_offset` of every buffer in
         `outs` (outs[0] on this device, the others peer-mapped buffers of other GPUs; tensors or raw pointers)"""
+        self._check_ntt_length(vec, log_n, batch)
         vec = vec.contiguous()
         ptrs = (ctypes.c_void_p * len(outs))(*[int(t) if isinstance(t, int) else int(t.data_ptr()) for t in outs])
         self._check(self.lib.sa_ntt_multi(ptrs, len(outs), out_offset, vec.data_ptr(), log_n, _limbs(root),
@@ -198,6 +208,7 @@ class CudaEngine:
     def ntt_mcast(self, mc_ptr, local, out_offset, vec, log_n, root, inverse=False, batch=1):
         """sa_ntt_mcast: transform `vec`, store the result through the multicast address `mc_ptr` (every rank's
         buffer receives it, this rank's `local` included) at element offset `out_offset`"""
+        self._check_ntt_length(vec, log_n, batch)
         vec = vec.contiguous()
         self._check(self.lib.sa_ntt_mcast(ctypes.c_void_p(int(mc_ptr)), local.data_ptr(), out_offset, vec.data_ptr(),
                                           log_n, _limbs(root), int(bool(inverse)), batch, self._stream()))
