@@ -143,8 +143,25 @@ int sa_zerofier(void *out, const void *domain, size_t k, void *stream);
  * < k with value values[i] at domain[i], k <= 2^20.  SA_EDIVZERO when two domain points coincide
  * (the reference's element-wise division asserts there).  Small k: Lagrange kernels; larger k:
  * zerofier tree, weights v_i / M'(d_i), and a bottom-up combination over the same tree - one call,
- * everything on the device.  Synchronises.                                                    */
+ * everything on the device.  Synchronises.  It is sa_interp_plan into a per-stream workspace
+ * followed by sa_interp_apply.                                                                */
 int sa_interpolate(void *out, const void *domain, const void *values, size_t k, void *stream);
+/* Interpolation plans: the part of sa_interpolate that depends on the domain alone (the zerofier tree
+ * and 1/M'(d_i)), built once and applied to any number of value vectors over the same domain.
+ * The plan is a device buffer the caller owns, of sa_interp_plan_bytes(k) bytes; its layout is
+ * internal and depends on k alone (656 MiB at k = 2^20).
+ * sa_interp_plan_bytes: 0 when k == 0 or k > 2^20.  Host-only: no CUDA call.                  */
+size_t sa_interp_plan_bytes(size_t k);
+/* Builds the plan of domain[0..k).  SA_ESIZE for k == 0 or k > 2^20, SA_EDIVZERO when two domain
+ * points coincide.  Synchronises (it reads the zero flag).                                    */
+int sa_interp_plan(void *plan, const void *domain, size_t k, void *stream);
+/* out[0..k) = the coefficients sa_interpolate gives for values[0..k) over the plan's domain; k must
+ * be the plan's k.  Asynchronous: no host synchronisation, and no allocation once the stream's
+ * workspace has grown to this size, so the call can be captured in a CUDA graph after one call on
+ * the capturing stream (the graph keeps that stream's workspace: replay it where that stream's other
+ * work cannot run concurrently, and make no larger call on that stream while the graph is in use).
+ * Reads the plan only: one plan may be applied on several streams at once.                    */
+int sa_interp_apply(void *out, const void *plan, const void *values, size_t k, void *stream);
 
 /* ---- code/merkle.py:6-14 Merkle.commit -------------------------------------------------
  * Builds the whole blake2b-512 tree over n = 2^k leaves, leaf = H(decimal ASCII of the

@@ -17,8 +17,10 @@ __global__ void k_pointwise_mul(fe *out, const fe *a, const fe *b, long long n) 
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
         tile_st(out + i, fe_montmul(fe_to_mont(tile_ld(a + i)), tile_ld(b + i)));
 }
-// out = a / b with Montgomery's batch-inversion trick over 8 strided elements per thread
-__global__ void k_pointwise_div(fe *out, const fe *a, const fe *b, long long n, int *zero_flag) {
+// Montgomery's batch-inversion trick over 8 strided elements per thread (one Fermat inverse per 8 elements):
+// emit(i, Montgomery form of 1/b[i]) for every i < n; a zero b[i] raises *zero_flag and is inverted as 1
+template <class Emit>
+__device__ __forceinline__ void batch_inverse(const fe *b, long long n, int *zero_flag, Emit emit) {
     constexpr int G = 8;
     const long long stride = (long long)gridDim.x * blockDim.x;
     const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -41,11 +43,19 @@ __global__ void k_pointwise_div(fe *out, const fe *a, const fe *b, long long n, 
 #pragma unroll
         for (int g = G - 1; g >= 0; g--) {
             const long long i = base + g * stride;
-            const fe binv = fe_montmul(inv, pre[g]);  // Montgomery form of 1/b[i]
+            const fe binv = fe_montmul(inv, pre[g]);
             inv = fe_montmul(inv, bm[g]);
-            if (i < n) tile_st(out + i, fe_montmul(tile_ld(a + i), binv));
+            if (i < n) emit(i, binv);
         }
     }
+}
+// out = a / b
+__global__ void k_pointwise_div(fe *out, const fe *a, const fe *b, long long n, int *zero_flag) {
+    batch_inverse(b, n, zero_flag, [&](long long i, const fe &binv) { tile_st(out + i, fe_montmul(tile_ld(a + i), binv)); });
+}
+// inv_m[i] = Montgomery form of 1/b[i]: the interpolation plan's 1/M'(d_i)
+__global__ void k_batch_inverse(fe *inv_m, const fe *b, long long n, int *zero_flag) {
+    batch_inverse(b, n, zero_flag, [&](long long i, const fe &binv) { tile_st(inv_m + i, binv); });
 }
 // out[i] = in[i] * factor^i; thread handles i, i + T, i + 2T, ... with running factor^T
 __global__ void k_scale(fe *out, const fe *in, long long n, fe factor_m, fe factor_T_m) {
@@ -101,7 +111,8 @@ __global__ void __launch_bounds__(ZF_THREADS) k_zerofier(fe *out, const fe *doma
 }
 // Lagrange interpolation pieces.  q_i = z / (X - d_i) by synthetic division (descending m):
 //   q_i[m-1] = z[m] + d_i * q_i[m];  D_i = q_i(d_i) = z'(d_i);  weight w_i = v_i / D_i
-__global__ void k_interp_weights(fe *w_m, const fe *domain, const fe *values, const fe *z, int k, int *zero_flag) {
+// dinv_m[i] = Montgomery form of 1/D_i (the plan's part: it depends on the domain only)
+__global__ void k_interp_weights(fe *dinv_m, const fe *domain, const fe *z, int k, int *zero_flag) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= k) return;
     const fe d = fe_to_mont(tile_ld(domain + i));
@@ -114,13 +125,13 @@ __global__ void k_interp_weights(fe *w_m, const fe *domain, const fe *values, co
         *zero_flag = 1;
         denom = fe_one();
     }
-    tile_st(w_m + i, fe_montmul(fe_to_mont(tile_ld(values + i)), fe_mont_inv(fe_to_mont(denom))));
+    tile_st(dinv_m + i, fe_mont_inv(fe_to_mont(denom)));
 }
-// QT[m][i] = w_i * q_i[m]  (coalesced over i)
-__global__ void k_interp_rows(fe *QT, const fe *domain, const fe *w_m, const fe *z, int k) {
+// QT[m][i] = w_i * q_i[m], w_i = v_i / D_i  (coalesced over i)
+__global__ void k_interp_rows(fe *QT, const fe *domain, const fe *dinv_m, const fe *values, const fe *z, int k) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= k) return;
-    const fe d = fe_to_mont(tile_ld(domain + i)), w = tile_ld(w_m + i);
+    const fe d = fe_to_mont(tile_ld(domain + i)), w = fe_montmul(fe_to_mont(tile_ld(values + i)), tile_ld(dinv_m + i));
     fe carry = fe_zero();
     for (int m = k; m > 0; m--) {
         carry = fe_add(tile_ldg(z + m), fe_montmul(carry, d));
@@ -210,10 +221,11 @@ __global__ void k_derivative(fe *out, const fe *z, long long k) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < k) tile_st(out + i, fe_montmul(fe_to_mont(fe_from_u64((uint64_t)(i + 1))), tile_ld(z + i + 1)));
 }
-// leaves of the interpolation sweep: q_i = v_i / M'(d_i) for i < k, 0 for the empty slots
-__global__ void k_tree_qleaves(fe *P0, const fe *q, long long k, long long K) {
+// leaves of the interpolation sweep: q_i = v_i / M'(d_i) for i < k (inv_m = the plan's Montgomery 1/M'(d_i)),
+// 0 for the empty slots
+__global__ void k_tree_qleaves(fe *P0, const fe *values, const fe *inv_m, long long k, long long K) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < K) tile_st(P0 + i, i < k ? tile_ld(q + i) : fe_zero());
+    if (i < K) tile_st(P0 + i, i < k ? fe_montmul(tile_ld(values + i), tile_ld(inv_m + i)) : fe_zero());
 }
 // zerofier coefficients from the tree's root vector: k == K -> implied leading 1
 __global__ void k_tree_root(fe *out, const fe *root, long long k, long long K) {
@@ -412,19 +424,23 @@ static int tree_build(PolyTree &t, const fe *domain, cudaStream_t st) {
     }
     return SA_OK;
 }
-static int tree_alloc(PolyTree &t, size_t k, bool keep_transforms, size_t extra_elems, fe **extra, cudaStream_t st) {
+// keep_transforms: every level's node transforms stay (logK * 2K elements, read by the walk down and the up-sweep),
+// in `transforms` when the caller gives a buffer (an interpolation plan), else in the workspace
+static int tree_alloc(PolyTree &t, size_t k, bool keep_transforms, size_t extra_elems, fe **extra, cudaStream_t st,
+                      fe *transforms = nullptr) {
     t.k = (long long)k;
     t.logK = 0;
     while ((size_t(1) << t.logK) < k) t.logK++;
     if (t.logK > TREE_MAX_LOG) return SA_ESIZE;
     t.K = 1ll << t.logK;
     const size_t K = (size_t)t.K;
-    const size_t lv = (size_t)(t.logK + 1) * K, tr = keep_transforms ? (size_t)t.logK * 2 * K : 0, sc = 2 * K;
+    const bool in_ws = keep_transforms && !transforms;
+    const size_t lv = (size_t)(t.logK + 1) * K, tr = in_ws ? (size_t)t.logK * 2 * K : 0, sc = 2 * K;
     fe *ws = nullptr;
     int rc = get_workspace((void **)&ws, sizeof(fe) * (lv + tr + sc + extra_elems), st, 8);
     if (rc != SA_OK) return rc;
     t.levels = ws;
-    t.transforms = keep_transforms ? ws + lv : nullptr;
+    t.transforms = in_ws ? ws + lv : keep_transforms ? transforms : nullptr;
     t.scratch = ws + lv + tr;
     if (extra) *extra = ws + lv + tr + sc;
     return SA_OK;
@@ -524,46 +540,62 @@ int sa_zerofier(void *out, const void *domain, size_t k, void *stream) {
     return SA_OK;
 }
 
-static int interpolate_direct(void *out, const void *domain, const void *values, size_t k, cudaStream_t st) {
-    // workspace: z (k+1) | w (k) | flag | QT (k*k)
-    char *ws = nullptr;
-    const size_t z_off = 0, w_off = sizeof(fe) * (k + 1), f_off = w_off + sizeof(fe) * k,
-                 q_off = f_off + 16, total = q_off + sizeof(fe) * k * k;
-    int rc = get_workspace((void **)&ws, total, st, 7);
-    if (rc != SA_OK) return rc;
-    fe *z = (fe *)(ws + z_off), *w = (fe *)(ws + w_off), *QT = (fe *)(ws + q_off);
-    int *flag = (int *)(ws + f_off);
-    if ((rc = sa_zerofier(z, domain, k, (void *)st)) != SA_OK) return rc;
-    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
-    const int bs = 128, grid = (int)((k + bs - 1) / bs);
-    k_interp_weights<<<grid, bs, 0, st>>>(w, (const fe *)domain, (const fe *)values, z, (int)k, flag);
-    SA_LAUNCH_CHECK();
-    k_interp_rows<<<grid, bs, 0, st>>>(QT, (const fe *)domain, w, z, (int)k);
-    SA_LAUNCH_CHECK();
-    k_interp_colsum<<<(unsigned)k, 256, 0, st>>>((fe *)out, QT, (int)k);
-    SA_LAUNCH_CHECK();
-    int h = 0;
-    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    SA_CUDA(cudaStreamSynchronize(st));
-    return h ? SA_EDIVZERO : SA_OK;
+// ---- interpolation plans: the half of fast_interpolate (ntt.py:102-130) that depends on the domain alone ----
+// A plan is a device buffer of sa_interp_plan_bytes(k) bytes, laid out by k alone.  Every section starts on a
+// 256-byte (16-element) boundary, i.e. each section's length is rounded up to a multiple of 16 elements:
+//   k <= g_interp_direct_max (the k x k Lagrange kernels):  domain (k) | z = prod (X - d_i) (k + 1) | 1/z'(d_i) (k)
+//   above (the subproduct tree):  node transforms of levels 0 .. log K - 1, as tree_build keeps them (log K * 2K)
+//                                 | 1/M'(d_i) (K; the first k are written)
+// The inverses are in Montgomery form, so one product per point gives v_i / M'(d_i).  The tree's levels and z stay
+// in the build's workspace: the up-sweep reads the node transforms only.  2^20 points: 41 * 2^20 elements, 656 MiB.
+struct InterpPlan {
+    bool direct = false;
+    int logK = 0;
+    long long K = 0;
+    size_t sec[3] = {0, 0, 0};  // element offsets: domain, z, 1/z'  |  transforms, 1/M'
+    size_t elems = 0;           // 0: no plan for this k
+};
+static inline size_t plan_section(size_t elems) { return (elems + 15) & ~(size_t)15; }
+static InterpPlan interp_plan_layout(size_t k) {
+    InterpPlan L;
+    tree_config();
+    if (k == 0 || k > ((size_t)1 << TREE_MAX_LOG)) return L;
+    L.direct = k <= (size_t)g_interp_direct_max && k <= (size_t)ZF_MAXK;
+    if (L.direct) {
+        L.sec[1] = plan_section(k);
+        L.sec[2] = L.sec[1] + plan_section(k + 1);
+        L.elems = L.sec[2] + plan_section(k);
+    } else {
+        L.logK = host_log2(k);
+        L.K = 1ll << L.logK;
+        L.sec[1] = plan_section((size_t)L.logK * 2 * (size_t)L.K);
+        L.elems = L.sec[1] + plan_section((size_t)L.K);
+    }
+    return L;
 }
-
-// Lagrange interpolation through the subproduct tree, everything on the device:
-//   M = prod (X - d_i) (tree), q_i = v_i / M'(d_i), and the interpolant sum_i q_i M / (X - d_i) is
-//   combined bottom-up: P_node = P_L * M_R + P_R * M_L (the M's are the tree's nodes, their transforms
-//   kept from the build).  M'(d_i) comes from one Horner kernel (k^2 / 2 multiply-adds, all points in
-//   parallel); coinciding points give M'(d_i) = 0 -> SA_EDIVZERO like the division at ntt.py:124-125.
-static int interpolate_tree(void *out, const void *domain, const void *values, size_t k, cudaStream_t st) {
+static int interp_plan_direct(fe *plan, const InterpPlan &L, const fe *domain, size_t k, int *flag, cudaStream_t st) {
+    fe *z = plan + L.sec[1];
+    SA_CUDA(cudaMemcpyAsync(plan, domain, sizeof(fe) * k, cudaMemcpyDeviceToDevice, st));
+    int rc = sa_zerofier(z, domain, k, (void *)st);
+    if (rc != SA_OK) return rc;
+    const int bs = 128, grid = (int)((k + bs - 1) / bs);
+    k_interp_weights<<<grid, bs, 0, st>>>(plan + L.sec[2], domain, z, (int)k, flag);
+    SA_LAUNCH_CHECK();
+    return SA_OK;
+}
+// M = prod (X - d_i) by the tree (its node transforms go into the plan), M'(d_i) from one Horner kernel (k^2 / 2
+// multiply-adds, all points in parallel) or, from 2^13.75 points, the walk down the tree, then one batch inversion;
+// coinciding points give M'(d_i) = 0 -> the zero flag (SA_EDIVZERO like the division at ntt.py:124-125)
+static int interp_plan_tree(fe *plan, const InterpPlan &L, const fe *domain, size_t k, int *flag, cudaStream_t st) {
     PolyTree t;
     fe *extra = nullptr;
-    // extra: z (K + 1) | dz (K) | ev (K) | q (K) | P levels ping-pong (2 * K)
-    const size_t Kpad = (size_t)1 << (k <= 1 ? 0 : (64 - __builtin_clzll((unsigned long long)(k - 1))));
+    const size_t K = (size_t)L.K;
     const bool walk = (double)k * (double)k >= g_eval_tree_min;  // M'(d_i): Horner is k^2 products
-    int rc = tree_alloc(t, k, true, 6 * Kpad + 16 + (walk ? multipoint_extra(k, k) : 0), &extra, st);
+    // extra: z (K + 1) | dz (K) | ev (K) | the walk's workspace
+    int rc = tree_alloc(t, k, true, 3 * K + 1 + (walk ? multipoint_extra(k, k) : 0), &extra, st, plan + L.sec[0]);
     if (rc != SA_OK) return rc;
-    const size_t K = (size_t)t.K;
-    fe *z = extra, *dz = z + K + 1, *ev = dz + K, *q = ev + K, *Pa = q + K, *Pb = Pa + K, *mp = Pb + K + 16;
-    if ((rc = tree_build(t, (const fe *)domain, st)) != SA_OK) return rc;
+    fe *z = extra, *dz = z + K + 1, *ev = dz + K, *mp = ev + K;
+    if ((rc = tree_build(t, domain, st)) != SA_OK) return rc;
     k_tree_root<<<(unsigned)((k + 1 + 255) / 256), 256, 0, st>>>(z, t.levels + (size_t)t.logK * K, t.k, t.K);
     SA_LAUNCH_CHECK();
     k_derivative<<<(unsigned)((k + 255) / 256), 256, 0, st>>>(dz, z, (long long)k);
@@ -573,21 +605,64 @@ static int interpolate_tree(void *out, const void *domain, const void *values, s
     else
         rc = poly_eval_horner(ev, dz, k, domain, k, (void *)st);
     if (rc != SA_OK) return rc;
-    if ((rc = sa_pointwise_div(q, values, ev, k, (void *)st)) != SA_OK) return rc;  // SA_EDIVZERO: repeated point
-    k_tree_qleaves<<<(unsigned)((K + 255) / 256), 256, 0, st>>>(Pa, q, t.k, t.K);
+    k_batch_inverse<<<grid_for(((long long)k + 7) / 8, 128), 128, 0, st>>>(plan + L.sec[1], ev, (long long)k, flag);
     SA_LAUNCH_CHECK();
-    fe *cur = Pa, *nxt = Pb;
-    for (int j = 0; j < t.logK; j++) {
+    return SA_OK;
+}
+
+size_t sa_interp_plan_bytes(size_t k) { return sizeof(fe) * interp_plan_layout(k).elems; }
+
+int sa_interp_plan(void *plan, const void *domain, size_t k, void *stream) {
+    const InterpPlan L = interp_plan_layout(k);
+    if (L.elems == 0) return SA_ESIZE;
+    cudaStream_t st = (cudaStream_t)stream;
+    int *flag = nullptr;
+    int rc = get_workspace((void **)&flag, 16, st, 7);
+    if (rc != SA_OK) return rc;
+    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+    rc = L.direct ? interp_plan_direct((fe *)plan, L, (const fe *)domain, k, flag, st)
+                  : interp_plan_tree((fe *)plan, L, (const fe *)domain, k, flag, st);
+    if (rc != SA_OK) return rc;
+    int h = 0;
+    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SA_CUDA(cudaStreamSynchronize(st));
+    return h ? SA_EDIVZERO : SA_OK;
+}
+
+// Reads the plan only; its scratch is the stream's workspace (tag 10): QT (k * k) for the Lagrange kernels, the
+// up-sweep's transform scratch (2K) and P levels ping-pong (2 * K) above them.
+int sa_interp_apply(void *out, const void *plan, const void *values, size_t k, void *stream) {
+    const InterpPlan L = interp_plan_layout(k);
+    if (L.elems == 0) return SA_ESIZE;
+    cudaStream_t st = (cudaStream_t)stream;
+    const fe *p = (const fe *)plan, *v = (const fe *)values;
+    const size_t K = (size_t)L.K;
+    fe *ws = nullptr;
+    int rc = get_workspace((void **)&ws, sizeof(fe) * (L.direct ? k * k : 4 * K), st, 10);
+    if (rc != SA_OK) return rc;
+    if (L.direct) {
+        const int bs = 128, grid = (int)((k + bs - 1) / bs);
+        k_interp_rows<<<grid, bs, 0, st>>>(ws, p, p + L.sec[2], v, p + L.sec[1], (int)k);
+        SA_LAUNCH_CHECK();
+        k_interp_colsum<<<(unsigned)k, 256, 0, st>>>((fe *)out, ws, (int)k);
+        SA_LAUNCH_CHECK();
+        return SA_OK;
+    }
+    // the interpolant sum_i q_i M / (X - d_i), q_i = v_i / M'(d_i), combined bottom-up: P_node = P_L * M_R + P_R * M_L
+    fe *scratch = ws, *cur = ws + 2 * K, *nxt = cur + K;
+    k_tree_qleaves<<<(unsigned)((K + 255) / 256), 256, 0, st>>>(cur, v, p + L.sec[1], (long long)k, L.K);
+    SA_LAUNCH_CHECK();
+    for (int j = 0; j < L.logK; j++) {
         uint64_t root[2];
         tree_root_of_unity(root, j + 1);
-        const fe *VT = t.transforms + (size_t)j * 2 * K;
-        k_tree_pad<<<tree_grid(2 * (long long)K), 256, 0, st>>>(t.scratch, cur, t.K, j);
+        const fe *VT = p + L.sec[0] + (size_t)j * 2 * K;
+        k_tree_pad<<<tree_grid(2 * L.K), 256, 0, st>>>(scratch, cur, L.K, j);
         SA_LAUNCH_CHECK();
-        if ((rc = sa_ntt(t.scratch, t.scratch, j + 1, root, 0, K >> j, (void *)st)) != SA_OK) return rc;
-        k_tree_cross<<<tree_grid((long long)K), 256, 0, st>>>(nxt, t.scratch, VT, t.K, j);
+        if ((rc = sa_ntt(scratch, scratch, j + 1, root, 0, K >> j, (void *)st)) != SA_OK) return rc;
+        k_tree_cross<<<tree_grid(L.K), 256, 0, st>>>(nxt, scratch, VT, L.K, j);
         SA_LAUNCH_CHECK();
         if ((rc = sa_ntt(nxt, nxt, j + 1, root, 1, K >> (j + 1), (void *)st)) != SA_OK) return rc;
-        k_tree_fix<<<tree_grid((long long)K / 2), 256, 0, st>>>(nxt, cur, t.K, j, t.k, 1);
+        k_tree_fix<<<tree_grid(L.K / 2), 256, 0, st>>>(nxt, cur, L.K, j, (long long)k, 1);
         SA_LAUNCH_CHECK();
         fe *tmp = cur;
         cur = nxt;
@@ -597,13 +672,16 @@ static int interpolate_tree(void *out, const void *domain, const void *values, s
     return SA_OK;
 }
 
+// plan (per-stream workspace, tag 9) + apply: one implementation for the one-shot call and for plans
 int sa_interpolate(void *out, const void *domain, const void *values, size_t k, void *stream) {
     if (k == 0) return SA_OK;
-    tree_config();
-    cudaStream_t st = (cudaStream_t)stream;
-    if (k <= (size_t)g_interp_direct_max && k <= (size_t)ZF_MAXK) return interpolate_direct(out, domain, values, k, st);
-    if (k > ((size_t)1 << TREE_MAX_LOG)) return SA_ESIZE;
-    return interpolate_tree(out, domain, values, k, st);
+    const size_t bytes = sa_interp_plan_bytes(k);
+    if (bytes == 0) return SA_ESIZE;
+    void *plan = nullptr;
+    int rc = get_workspace(&plan, bytes, (cudaStream_t)stream, 9);
+    if (rc != SA_OK) return rc;
+    if ((rc = sa_interp_plan(plan, domain, k, stream)) != SA_OK) return rc;
+    return sa_interp_apply(out, plan, values, k, stream);
 }
 
 // fast_evaluate (ntt.py:82-100): Horner for small jobs, the transposed tree walk (tree_multipoint) for big ones

@@ -56,6 +56,9 @@ SYMBOLS = [
     ("sa_poly_eval_mode", _ci, [_vp, _vp, _sz, _vp, _sz, _ci, _vp]),
     ("sa_zerofier", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_interpolate", _ci, [_vp, _vp, _vp, _sz, _vp]),
+    ("sa_interp_plan_bytes", _sz, [_sz]),
+    ("sa_interp_plan", _ci, [_vp, _vp, _sz, _vp]),
+    ("sa_interp_apply", _ci, [_vp, _vp, _vp, _sz, _vp]),
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
@@ -91,6 +94,16 @@ def _limbs(x):
 
 class SaError(AssertionError):
     """Raised with the reference's assertion message for SA_E* codes."""
+
+
+class InterpPlan:
+    """An interpolation plan (CudaEngine.interp_plan): the device buffer sa_interp_plan filled (torch.uint8) for a
+    domain of k points."""
+    __slots__ = ("plan", "k")
+
+    def __init__(self, plan, k):
+        self.plan = plan
+        self.k = k
 
 
 class CudaEngine:
@@ -259,6 +272,26 @@ class CudaEngine:
         out = self.empty(domain.shape[0])
         self._check(self.lib.sa_interpolate(out.data_ptr(), domain.data_ptr(), values.data_ptr(), domain.shape[0],
                                             self._stream()))
+        return out
+
+    def interp_plan(self, domain):
+        """sa_interp_plan: what interpolation over `domain` needs of the domain alone, kept on the device for
+        interp_apply (synchronises; "divide by zero" when two points coincide)"""
+        domain = domain.contiguous()
+        k = domain.shape[0]
+        plan = self.torch.empty(self.lib.sa_interp_plan_bytes(k), dtype=self.torch.uint8, device=self.device)
+        self._check(self.lib.sa_interp_plan(plan.data_ptr(), domain.data_ptr(), k, self._stream()))
+        return InterpPlan(plan, k)
+
+    def interp_apply(self, plan, values):
+        """sa_interp_apply: the coefficients `interpolate` gives for `values` over the plan's domain; asynchronous,
+        the plan is only read"""
+        if values.shape[0] != plan.k:  # the library cannot see the vector's length
+            raise SaError(SA_ERRORS[-6])
+        values = values.contiguous()
+        out = self.empty(plan.k)
+        self._check(self.lib.sa_interp_apply(out.data_ptr(), plan.plan.data_ptr(), values.data_ptr(), plan.k,
+                                             self._stream()))
         return out
 
     # --------------------------------------------------------------- merkle
