@@ -160,8 +160,25 @@ int sa_interp_plan(void *plan, const void *domain, size_t k, void *stream);
  * workspace has grown to this size, so the call can be captured in a CUDA graph after one call on
  * the capturing stream (the graph keeps that stream's workspace: replay it where that stream's other
  * work cannot run concurrently, and make no larger call on that stream while the graph is in use).
- * Reads the plan only: one plan may be applied on several streams at once.                    */
+ * Reads the plan only: one plan may be applied on several streams at once.  It is
+ * sa_interp_apply_batch with batch 1.                                                         */
 int sa_interp_apply(void *out, const void *plan, const void *values, size_t k, void *stream);
+/* out[b*k .. b*k+k) = the coefficients sa_interp_apply gives for values[b*k .. b*k+k), b < batch:
+ * many value vectors over one plan's domain in one call.  Rows are contiguous; out must not
+ * overlap values.  batch == 0 returns SA_OK without a launch, a k outside 1..2^20 gives SA_ESIZE.
+ * The same promises as sa_interp_apply: plan only read, no host synchronisation, and no
+ * allocation once the stream's workspaces have grown for this k and chunk size.  Up to 1024
+ * points the batch is one field matrix product (2 launches, k^2 elements of workspace whatever
+ * the batch size); above, every level of the up-sweep is one batch over all vectors' nodes, in
+ * chunks of sa_interp_batch_max(k) vectors, each chunk issuing the launches of one
+ * sa_interp_apply.  A chunk takes 96 bytes per leaf slot (K = 2^ceil(log2 k) slots) per vector
+ * of per-stream workspace.                                                                    */
+int sa_interp_apply_batch(void *out, const void *plan, const void *values, size_t k, size_t batch, void *stream);
+/* The most vectors one chunk of sa_interp_apply_batch takes for a k-point plan: SIZE_MAX up to
+ * 1024 points (one pass whatever the batch), max(1, floor(2^30 / (96 K))) above (a chunk's
+ * workspace stays at or below 1 GiB: 10 vectors at 2^20, 170 at 2^16), 0 when k == 0 or
+ * k > 2^20.  Host-only: no CUDA call.                                                         */
+size_t sa_interp_batch_max(size_t k);
 
 /* ---- code/merkle.py:6-14 Merkle.commit -------------------------------------------------
  * Builds the whole blake2b-512 tree over n = 2^k leaves, leaf = H(decimal ASCII of the

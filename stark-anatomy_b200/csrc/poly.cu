@@ -3,6 +3,7 @@
 // sa_poly_eval.
 //
 // Reference behaviour reproduced (bit-exact): code/ntt.py:61-172, code/algebra.py:53-57,75-94.
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <mutex>
@@ -127,31 +128,71 @@ __global__ void k_interp_weights(fe *dinv_m, const fe *domain, const fe *z, int 
     }
     tile_st(dinv_m + i, fe_mont_inv(fe_to_mont(denom)));
 }
-// QT[m][i] = w_i * q_i[m], w_i = v_i / D_i  (coalesced over i)
-__global__ void k_interp_rows(fe *QT, const fe *domain, const fe *dinv_m, const fe *values, const fe *z, int k) {
+// QT[m][i] = q_i[m] / D_i, the Lagrange basis polynomials' coefficients, in Montgomery form like the twiddles
+// (coalesced over i; domain only)
+__global__ void k_interp_rows(fe *QT, const fe *domain, const fe *dinv_m, const fe *z, int k) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= k) return;
-    const fe d = fe_to_mont(tile_ld(domain + i)), w = fe_montmul(fe_to_mont(tile_ld(values + i)), tile_ld(dinv_m + i));
+    const fe d = fe_to_mont(tile_ld(domain + i)), w = fe_to_mont(tile_ld(dinv_m + i));
     fe carry = fe_zero();
     for (int m = k; m > 0; m--) {
         carry = fe_add(tile_ldg(z + m), fe_montmul(carry, d));
         tile_st(QT + (size_t)(m - 1) * k + i, fe_montmul(carry, w));
     }
 }
-// out[m] = sum_i QT[m][i]; one CTA per coefficient
-__global__ void __launch_bounds__(256) k_interp_colsum(fe *out, const fe *QT, int k) {
-    __shared__ uint4 red_u4[256];
-    fe *red = reinterpret_cast<fe *>(red_u4);
-    const int m = blockIdx.x, tid = threadIdx.x;
-    fe acc = fe_zero();
-    for (int i = tid; i < k; i += 256) acc = fe_add(acc, tile_ld(QT + (size_t)m * k + i));
-    red[tid] = acc;
-    __syncthreads();
-    for (int w = 128; w >= 1; w >>= 1) {
-        if (tid < w) red[tid] = fe_add(red[tid], red[tid + w]);
-        __syncthreads();
+__device__ __forceinline__ fe fe_shfl_down(const fe &x, int off) {
+    fe y;
+#pragma unroll
+    for (int j = 0; j < 4; j++) y.v[j] = __shfl_down_sync(0xffffffffu, x.v[j], off);
+    return y;
+}
+// out[b][m] = sum_i V[b][i] * QT[m][i], b < B, m < k: the Lagrange sums of B value vectors as one field matrix
+// product.  A CTA owns IM_TB vectors x IM_TM coefficients and all its threads split the sum over i, so a single
+// vector still spreads over k / IM_TM CTAs: each thread keeps IM_TB x IM_TM partial sums in registers (every V
+// element it loads serves IM_TM products, every QT element IM_TB; QT is in Montgomery form, so a product is one
+// fe_montmul), then the warps add theirs by shuffles and the CTA through shared memory.
+constexpr int IM_TM = 2, IM_TB = 4, IM_THREADS = 256;
+__global__ void __launch_bounds__(IM_THREADS) k_interp_matmul(fe *out, const fe *V, const fe *QT, int k, long long B) {
+    __shared__ uint4 red_u4[IM_THREADS / 32][IM_TB * IM_TM];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const long long b0 = (long long)blockIdx.x * IM_TB;
+    const int m0 = blockIdx.y * IM_TM, nb = (int)(B - b0 < IM_TB ? B - b0 : IM_TB);
+    fe acc[IM_TB][IM_TM];
+#pragma unroll
+    for (int r = 0; r < IM_TB; r++)
+#pragma unroll
+        for (int c = 0; c < IM_TM; c++) acc[r][c] = fe_zero();
+    for (int i = tid; i < k; i += IM_THREADS) {
+        fe q[IM_TM];
+#pragma unroll
+        for (int c = 0; c < IM_TM; c++) q[c] = (m0 + c < k) ? tile_ld(QT + (size_t)(m0 + c) * k + i) : fe_zero();
+#pragma unroll
+        for (int r = 0; r < IM_TB; r++) {
+            if (r >= nb) break;
+            const fe v = tile_ld(V + (b0 + r) * k + i);
+#pragma unroll
+            for (int c = 0; c < IM_TM; c++) acc[r][c] = fe_add(acc[r][c], fe_montmul(v, q[c]));
+        }
     }
-    if (tid == 0) tile_st(out + m, red[0]);
+    fe *red = reinterpret_cast<fe *>(red_u4);
+#pragma unroll
+    for (int r = 0; r < IM_TB; r++) {
+        if (r >= nb) break;
+#pragma unroll
+        for (int c = 0; c < IM_TM; c++) {
+            fe s = acc[r][c];
+#pragma unroll
+            for (int off = 16; off >= 1; off >>= 1) s = fe_add(s, fe_shfl_down(s, off));
+            if (lane == 0) red[warp * IM_TB * IM_TM + r * IM_TM + c] = s;
+        }
+    }
+    __syncthreads();
+    const int r = tid / IM_TM, m = m0 + tid % IM_TM;
+    if (tid < IM_TB * IM_TM && r < nb && m < k) {
+        fe s = red[tid];
+        for (int w = 1; w < IM_THREADS / 32; w++) s = fe_add(s, red[w * IM_TB * IM_TM + tid]);
+        tile_st(out + (b0 + r) * k + m, s);
+    }
 }
 
 // ---- subproduct tree over a domain of k points (fast_zerofier / fast_interpolate, ntt.py:66-130) ----
@@ -184,25 +225,27 @@ __global__ void k_tree_pairmul(fe *out, const fe *in, long long K, int mlog) {
         tile_st(out + idx, fe_montmul(fe_to_mont(a), b));
     }
 }
-// interpolation up-sweep: out[p][t] = P[2p][t] * V[2p+1][t] + P[2p+1][t] * V[2p][t]
-__global__ void k_tree_cross(fe *out, const fe *Pt, const fe *Vt, long long K, int mlog) {
+// interpolation up-sweep of `batch` trees of K slots, back to back, over one tree's node transforms Vt (2K):
+// out[p][t] = P[2p][t] * V[2p+1][t] + P[2p+1][t] * V[2p][t]
+__global__ void k_tree_cross(fe *out, const fe *Pt, const fe *Vt, long long K, long long batch, int mlog) {
     const long long stride = (long long)gridDim.x * blockDim.x, two_m = 2ll << mlog;
-    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < K; idx += stride) {
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < batch * K; idx += stride) {
         const long long p = idx >> (mlog + 1), t = idx & (two_m - 1);
         const long long l = (2 * p) * two_m + t, r = (2 * p + 1) * two_m + t;
-        const fe a = fe_montmul(fe_to_mont(tile_ld(Pt + l)), tile_ld(Vt + r));
-        const fe b = fe_montmul(fe_to_mont(tile_ld(Pt + r)), tile_ld(Vt + l));
+        const fe a = fe_montmul(fe_to_mont(tile_ld(Pt + l)), tile_ld(Vt + (r & (2 * K - 1))));
+        const fe b = fe_montmul(fe_to_mont(tile_ld(Pt + r)), tile_ld(Vt + (l & (2 * K - 1))));
         tile_st(out + idx, fe_add(a, b));
     }
 }
 // parent[p][m + t] += [L full] right[t] + [R full] left[t]; (left, right) = the child vectors of `add`
 // (the zerofier tree adds the children's own vectors, the interpolation sweep the OTHER tree's: P_L * M_R
-// picks up x^m * P_L when M_R is full, so `swap` exchanges the roles)
-__global__ void k_tree_fix(fe *parent, const fe *add, long long K, int mlog, long long k, int swap) {
+// picks up x^m * P_L when M_R is full, so `swap` exchanges the roles).  `batch` trees of K slots, back to back:
+// a node is full by its index within its own tree.
+__global__ void k_tree_fix(fe *parent, const fe *add, long long K, long long batch, int mlog, long long k, int swap) {
     const long long stride = (long long)gridDim.x * blockDim.x, m = 1ll << mlog;
-    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < K / 2; idx += stride) {
-        const long long p = idx >> mlog, t = idx & (m - 1);
-        const bool lfull = tree_full(2 * p, mlog, k), rfull = tree_full(2 * p + 1, mlog, k);
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < batch * K / 2; idx += stride) {
+        const long long p = idx >> mlog, t = idx & (m - 1), left_node = (2 * p) & ((K >> mlog) - 1);
+        const bool lfull = tree_full(left_node, mlog, k), rfull = tree_full(left_node + 1, mlog, k);
         if (!lfull && !rfull) continue;
         const fe left = tile_ld(add + (2 * p) * m + t), right = tile_ld(add + (2 * p + 1) * m + t);
         fe acc = tile_ld(parent + p * 2 * m + m + t);
@@ -222,10 +265,12 @@ __global__ void k_derivative(fe *out, const fe *z, long long k) {
     if (i < k) tile_st(out + i, fe_montmul(fe_to_mont(fe_from_u64((uint64_t)(i + 1))), tile_ld(z + i + 1)));
 }
 // leaves of the interpolation sweep: q_i = v_i / M'(d_i) for i < k (inv_m = the plan's Montgomery 1/M'(d_i)),
-// 0 for the empty slots
-__global__ void k_tree_qleaves(fe *P0, const fe *values, const fe *inv_m, long long k, long long K) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < K) tile_st(P0 + i, i < k ? fe_montmul(tile_ld(values + i), tile_ld(inv_m + i)) : fe_zero());
+// 0 for the empty slots; vector b (values + b * k) fills the K = 2^logK slots at P0 + b * K
+__global__ void k_tree_qleaves(fe *P0, const fe *values, const fe *inv_m, long long k, int logK, long long batch) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= batch << logK) return;
+    const long long b = idx >> logK, i = idx & ((1ll << logK) - 1);
+    tile_st(P0 + idx, i < k ? fe_montmul(tile_ld(values + b * k + i), tile_ld(inv_m + i)) : fe_zero());
 }
 // zerofier coefficients from the tree's root vector: k == K -> implied leading 1
 __global__ void k_tree_root(fe *out, const fe *root, long long k, long long K) {
@@ -419,7 +464,7 @@ static int tree_build(PolyTree &t, const fe *domain, cudaStream_t st) {
         k_tree_pairmul<<<tree_grid(K), 256, 0, st>>>(parent, T, K, j);
         SA_LAUNCH_CHECK();
         if ((rc = sa_ntt(parent, parent, j + 1, root, 1, (size_t)(K >> (j + 1)), st)) != SA_OK) return rc;
-        k_tree_fix<<<tree_grid(K / 2), 256, 0, st>>>(parent, child, K, j, t.k, 0);
+        k_tree_fix<<<tree_grid(K / 2), 256, 0, st>>>(parent, child, K, 1, j, t.k, 0);
         SA_LAUNCH_CHECK();
     }
     return SA_OK;
@@ -629,47 +674,79 @@ int sa_interp_plan(void *plan, const void *domain, size_t k, void *stream) {
     return h ? SA_EDIVZERO : SA_OK;
 }
 
-// Reads the plan only; its scratch is the stream's workspace (tag 10): QT (k * k) for the Lagrange kernels, the
-// up-sweep's transform scratch (2K) and P levels ping-pong (2 * K) above them.
-int sa_interp_apply(void *out, const void *plan, const void *values, size_t k, void *stream) {
+// Above the Lagrange kernels a batched apply needs 4K elements of its own workspace (tag 10) and 2K of the NTT's
+// inter-pass intermediate (tag 0) per vector: 96K bytes.  It runs in chunks that keep both at or below 1 GiB.
+constexpr size_t INTERP_CHUNK_BYTES = (size_t)1 << 30;
+size_t sa_interp_batch_max(size_t k) {
     const InterpPlan L = interp_plan_layout(k);
-    if (L.elems == 0) return SA_ESIZE;
-    cudaStream_t st = (cudaStream_t)stream;
-    const fe *p = (const fe *)plan, *v = (const fe *)values;
+    if (L.elems == 0) return 0;
+    if (L.direct) return SIZE_MAX;
+    const size_t b = INTERP_CHUNK_BYTES / (sizeof(fe) * 6 * (size_t)L.K);
+    return b ? b : 1;
+}
+
+// the interpolants sum_i q_i M / (X - d_i), q_i = v_i / M'(d_i), of nb value vectors, combined bottom-up over the
+// plan's tree: P_node = P_L * M_R + P_R * M_L.  Every level is one batch over the nodes of all nb trees, so the
+// launches do not depend on nb.  ws = 4K * nb elements: transform scratch [nb][2K], P ping-pong 2 x [nb][K].
+static int interp_sweep(fe *out, const fe *p, const InterpPlan &L, const fe *v, size_t k, size_t nb, fe *ws,
+                        cudaStream_t st) {
     const size_t K = (size_t)L.K;
-    fe *ws = nullptr;
-    int rc = get_workspace((void **)&ws, sizeof(fe) * (L.direct ? k * k : 4 * K), st, 10);
-    if (rc != SA_OK) return rc;
-    if (L.direct) {
-        const int bs = 128, grid = (int)((k + bs - 1) / bs);
-        k_interp_rows<<<grid, bs, 0, st>>>(ws, p, p + L.sec[2], v, p + L.sec[1], (int)k);
-        SA_LAUNCH_CHECK();
-        k_interp_colsum<<<(unsigned)k, 256, 0, st>>>((fe *)out, ws, (int)k);
-        SA_LAUNCH_CHECK();
-        return SA_OK;
-    }
-    // the interpolant sum_i q_i M / (X - d_i), q_i = v_i / M'(d_i), combined bottom-up: P_node = P_L * M_R + P_R * M_L
-    fe *scratch = ws, *cur = ws + 2 * K, *nxt = cur + K;
-    k_tree_qleaves<<<(unsigned)((K + 255) / 256), 256, 0, st>>>(cur, v, p + L.sec[1], (long long)k, L.K);
+    const long long n = (long long)(nb * K);
+    fe *scratch = ws, *cur = ws + 2 * K * nb, *nxt = cur + K * nb;
+    int rc;
+    k_tree_qleaves<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cur, v, p + L.sec[1], (long long)k, L.logK,
+                                                                (long long)nb);
     SA_LAUNCH_CHECK();
     for (int j = 0; j < L.logK; j++) {
         uint64_t root[2];
         tree_root_of_unity(root, j + 1);
         const fe *VT = p + L.sec[0] + (size_t)j * 2 * K;
-        k_tree_pad<<<tree_grid(2 * L.K), 256, 0, st>>>(scratch, cur, L.K, j);
+        k_tree_pad<<<tree_grid(2 * n), 256, 0, st>>>(scratch, cur, n, j);
         SA_LAUNCH_CHECK();
-        if ((rc = sa_ntt(scratch, scratch, j + 1, root, 0, K >> j, (void *)st)) != SA_OK) return rc;
-        k_tree_cross<<<tree_grid(L.K), 256, 0, st>>>(nxt, scratch, VT, L.K, j);
+        if ((rc = sa_ntt(scratch, scratch, j + 1, root, 0, nb * (K >> j), (void *)st)) != SA_OK) return rc;
+        k_tree_cross<<<tree_grid(n), 256, 0, st>>>(nxt, scratch, VT, L.K, (long long)nb, j);
         SA_LAUNCH_CHECK();
-        if ((rc = sa_ntt(nxt, nxt, j + 1, root, 1, K >> (j + 1), (void *)st)) != SA_OK) return rc;
-        k_tree_fix<<<tree_grid(L.K / 2), 256, 0, st>>>(nxt, cur, L.K, j, (long long)k, 1);
+        if ((rc = sa_ntt(nxt, nxt, j + 1, root, 1, nb * (K >> (j + 1)), (void *)st)) != SA_OK) return rc;
+        k_tree_fix<<<tree_grid(n / 2), 256, 0, st>>>(nxt, cur, L.K, (long long)nb, j, (long long)k, 1);
         SA_LAUNCH_CHECK();
         fe *tmp = cur;
         cur = nxt;
         nxt = tmp;
     }
-    SA_CUDA(cudaMemcpyAsync(out, cur, sizeof(fe) * k, cudaMemcpyDeviceToDevice, st));
+    SA_CUDA(cudaMemcpy2DAsync(out, sizeof(fe) * k, cur, sizeof(fe) * K, sizeof(fe) * k, nb, cudaMemcpyDeviceToDevice,
+                              st));
     return SA_OK;
+}
+
+// Reads the plan only; its scratch is the stream's workspace (tag 10): Q' (k * k) for the Lagrange kernels, 4K per
+// vector of a chunk above them (see interp_sweep).
+int sa_interp_apply_batch(void *out, const void *plan, const void *values, size_t k, size_t batch, void *stream) {
+    const InterpPlan L = interp_plan_layout(k);
+    if (L.elems == 0) return SA_ESIZE;
+    if (batch == 0) return SA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const fe *p = (const fe *)plan, *v = (const fe *)values;
+    fe *o = (fe *)out, *ws = nullptr;
+    const size_t chunk = L.direct ? batch : std::min(batch, sa_interp_batch_max(k));
+    int rc = get_workspace((void **)&ws, sizeof(fe) * (L.direct ? k * k : 4 * (size_t)L.K * chunk), st, 10);
+    if (rc != SA_OK) return rc;
+    if (L.direct) {  // Q'[m][i] = q_i[m] / z'(d_i) from the plan, then out = V Q'^T
+        const int bs = 128, grid = (int)((k + bs - 1) / bs);
+        k_interp_rows<<<grid, bs, 0, st>>>(ws, p, p + L.sec[2], p + L.sec[1], (int)k);
+        SA_LAUNCH_CHECK();
+        const dim3 mgrid((unsigned)((batch + IM_TB - 1) / IM_TB), (unsigned)((k + IM_TM - 1) / IM_TM));
+        k_interp_matmul<<<mgrid, IM_THREADS, 0, st>>>(o, v, ws, (int)k, (long long)batch);
+        SA_LAUNCH_CHECK();
+        return SA_OK;
+    }
+    for (size_t b0 = 0; b0 < batch; b0 += chunk)
+        if ((rc = interp_sweep(o + b0 * k, p, L, v + b0 * k, k, std::min(chunk, batch - b0), ws, st)) != SA_OK)
+            return rc;
+    return SA_OK;
+}
+
+int sa_interp_apply(void *out, const void *plan, const void *values, size_t k, void *stream) {
+    return sa_interp_apply_batch(out, plan, values, k, 1, stream);
 }
 
 // plan (per-stream workspace, tag 9) + apply: one implementation for the one-shot call and for plans

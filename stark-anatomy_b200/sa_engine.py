@@ -59,6 +59,8 @@ SYMBOLS = [
     ("sa_interp_plan_bytes", _sz, [_sz]),
     ("sa_interp_plan", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_interp_apply", _ci, [_vp, _vp, _vp, _sz, _vp]),
+    ("sa_interp_apply_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _vp]),
+    ("sa_interp_batch_max", _sz, [_sz]),
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
@@ -284,14 +286,17 @@ class CudaEngine:
         return InterpPlan(plan, k)
 
     def interp_apply(self, plan, values):
-        """sa_interp_apply: the coefficients `interpolate` gives for `values` over the plan's domain; asynchronous,
-        the plan is only read"""
-        if values.shape[0] != plan.k:  # the library cannot see the vector's length
+        """sa_interp_apply_batch: the coefficients `interpolate` gives for `values` over the plan's domain, for one
+        vector (k, 2) or a batch of them (B, k, 2) in one call; asynchronous, the plan is only read"""
+        # the library cannot see the vectors' shape
+        if values.dim() not in (2, 3) or tuple(values.shape[-2:]) != (plan.k, 2):
             raise SaError(SA_ERRORS[-6])
         values = values.contiguous()
-        out = self.empty(plan.k)
-        self._check(self.lib.sa_interp_apply(out.data_ptr(), plan.plan.data_ptr(), values.data_ptr(), plan.k,
-                                             self._stream()))
+        out = self.torch.empty(values.shape, dtype=self.torch.int64, device=self.device)
+        batch = values.shape[0] if values.dim() == 3 else 1
+        if batch:
+            self._check(self.lib.sa_interp_apply_batch(out.data_ptr(), plan.plan.data_ptr(), values.data_ptr(), plan.k,
+                                                       batch, self._stream()))
         return out
 
     # --------------------------------------------------------------- merkle

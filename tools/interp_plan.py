@@ -9,10 +9,12 @@ Per domain size k, on random device-resident points and values, timed with CUDA 
   apply_ms           one sa_interp_apply (the value-dependent part; asynchronous)
   apply_x8_ms        8 applies of one plan to 8 value vectors, queued back to back (FastStark's 8 columns)
   interpolate_x8_ms  8 sa_interpolate calls on the same 8 vectors
+  apply_batchB_ms    one sa_interp_apply_batch of B vectors (--batch, default 8: the same 8 vectors as apply_x8_ms)
   plan_bytes         sa_interp_plan_bytes(k)
 
 apply_over_interpolate = apply_ms / interpolate_ms.  One JSON line per size, then one naming the device and its
-power limit (read in the same run).  Each size checks apply == sa_interpolate on its first vector."""
+power limit (read in the same run).  Each size checks apply == sa_interpolate on its first vector, and the batch's
+first and last rows against single applies."""
 import argparse
 import ctypes
 import json
@@ -67,6 +69,7 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--window", type=float, default=0.5, help="seconds per timed window")
     ap.add_argument("--sizes", type=int, nargs="*", default=SIZES)
+    ap.add_argument("--batch", type=int, default=8, help="vectors per sa_interp_apply_batch call")
     args = ap.parse_args()
 
     eng = sa_engine.get_engine()
@@ -101,9 +104,22 @@ def main():
                "apply_ms": timed_ms(apply, st, args.window),
                "apply_x8_ms": timed_ms(lambda: [apply(v) for v in vals], st, args.window),
                "interpolate_x8_ms": timed_ms(lambda: [interpolate(v) for v in vals], st, args.window)}
+        # after the single-vector columns, which thus run on the memory and workspaces they had before the batch
+        vbatch = torch.stack((vals + [rand_vec(k, dev) for _ in range(args.batch - 8)])[:args.batch])
+        obatch = torch.empty_like(vbatch)
+
+        def apply_batch():
+            assert lib.sa_interp_apply_batch(obatch.data_ptr(), plan.data_ptr(), vbatch.data_ptr(), k, args.batch,
+                                             stream) == 0
+
+        apply_batch()
+        for b in (0, args.batch - 1):
+            apply(vbatch[b])
+            assert bool((obatch[b] == out).all()), "batch row %d differs from a single apply at k = %d" % (b, k)
+        row["apply_batch%d_ms" % args.batch] = timed_ms(apply_batch, st, args.window)
         row["apply_over_interpolate"] = row["apply_ms"] / row["interpolate_ms"]
         print(json.dumps({key: (round(v, 4) if isinstance(v, float) else v) for key, v in row.items()}), flush=True)
-        del plan, dom, vals, out
+        del plan, dom, vals, out, vbatch, obatch
         torch.cuda.synchronize(dev)
         torch.cuda.empty_cache()
         assert lib.sa_release_workspaces() == 0
