@@ -255,7 +255,7 @@ int ntt_run(void *out, const void *in, int log_n, const uint64_t root[2], int in
         // its columns into registers before it writes any of them
         if (batch > (size_t)1 << 30) return SA_ESIZE;
     } else {
-        if ((rc = get_workspace((void **)&tmp, sizeof(fe) * n * batch, st)) != SA_OK) return rc;
+        if ((rc = get_workspace((void **)&tmp, sizeof(fe) * n * batch, st, WS_NTT)) != SA_OK) return rc;
         if (shape.l3 > 0 && batch * ((size_t)1 << (shape.l1 > shape.l2 ? shape.l1 : shape.l2)) > ((size_t)1 << 30))
             return SA_ESIZE;
     }
@@ -342,7 +342,7 @@ int sa_ntt_host(void *out_host, const void *in_host, int log_n, const uint64_t r
         // and an n-element intermediate per copy stream (32 GiB at 2^28): one transform at a time instead,
         // through one staging buffer on `st`
         void *dev = nullptr;
-        if ((rc = get_workspace(&dev, one, st, 1)) != SA_OK) return rc;
+        if ((rc = get_workspace(&dev, one, st, WS_HOST_STAGING)) != SA_OK) return rc;
         for (size_t b = 0; b < batch && rc == SA_OK; b++) {
             SA_CUDA(cudaMemcpyAsync(dev, (const char *)in_host + b * one, one, cudaMemcpyHostToDevice, st));
             rc = sa_ntt(dev, dev, log_n, root, inverse, 1, stream);
@@ -359,7 +359,7 @@ int sa_ntt_host(void *out_host, const void *in_host, int log_n, const uint64_t r
     const size_t nchunks = (batch + per_chunk - 1) / per_chunk;
     if (nchunks < 2) {
         void *dev = nullptr;
-        if ((rc = get_workspace(&dev, bytes, st, 1)) != SA_OK) return rc;
+        if ((rc = get_workspace(&dev, bytes, st, WS_HOST_STAGING)) != SA_OK) return rc;
         SA_CUDA(cudaMemcpyAsync(dev, in_host, bytes, cudaMemcpyHostToDevice, st));
         rc = sa_ntt(dev, dev, log_n, root, inverse, batch, stream);
         if (rc == SA_OK) SA_CUDA(cudaMemcpyAsync(out_host, dev, bytes, cudaMemcpyDeviceToHost, st));
@@ -392,7 +392,7 @@ int sa_ntt_host(void *out_host, const void *in_host, int log_n, const uint64_t r
     }
     void *buf[HOST_STREAMS_MAX];
     for (int i = 0; i < ns; i++)
-        if ((rc = get_workspace(&buf[i], per_chunk * one, g_copy_streams[i], 1)) != SA_OK) return rc;
+        if ((rc = get_workspace(&buf[i], per_chunk * one, g_copy_streams[i], WS_HOST_STAGING)) != SA_OK) return rc;
     SA_CUDA(cudaEventRecord(g_copy_events[ns], st));
     for (int i = 0; i < ns; i++) SA_CUDA(cudaStreamWaitEvent(g_copy_streams[i], g_copy_events[ns], 0));
     rc = SA_OK;

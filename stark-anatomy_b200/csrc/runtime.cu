@@ -16,7 +16,7 @@ std::atomic<uint64_t> g_launches{0};
 // intermediate and allocating it per call (even stream-ordered) costs more than the kernels.
 static std::mutex g_ws_mu;
 static std::map<std::tuple<int, cudaStream_t, int>, std::pair<void *, size_t>> g_ws;
-int get_workspace(void **out, size_t bytes, cudaStream_t st, int tag) {
+int get_workspace(void **out, size_t bytes, cudaStream_t st, WsTag tag) {
     int dev = 0;
     SA_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lock(g_ws_mu);

@@ -12,6 +12,7 @@
 
 #include "../../include/sa_b200.h"
 #include "field.cuh"
+#include "host.cuh"
 
 // ------------------------------------------------------------------ plumbing --
 extern thread_local std::string g_last_error;
@@ -34,13 +35,6 @@ extern std::atomic<uint64_t> g_launches;
             return SA_ECUDA;                                                                   \
         }                                                                                      \
     } while (0)
-
-static inline bool host_is_pow2(size_t n) { return n && !(n & (n - 1)); }
-static inline int host_log2(size_t n) {
-    int l = 0;
-    while ((size_t(1) << l) < n) l++;
-    return l;
-}
 
 // kernels with more than 48 KB of dynamic shared memory need the opt-in once per (kernel, device)
 constexpr int SA_MAX_DEVICES = 64;
@@ -83,8 +77,18 @@ static inline unsigned grid_for(long long n, int bs, int per_sm = 16) {
 }
 
 // ------------------------------------------------------------- workspaces --
-// grow-only scratch buffer `tag` of (current device, st)
-int get_workspace(void **out, size_t bytes, cudaStream_t st, int tag = 0);
+// grow-only scratch buffer `tag` of (current device, st).  Growing a buffer frees the old one, so a call never
+// takes a tag that it or its caller still holds; distinct tags nest: sa_interpolate holds WS_INTERP_PLAN across
+// the plan build (WS_PLAN_FLAG, WS_TREE) and the apply (WS_INTERP_APPLY), and every sa_ntt inside them takes WS_NTT.
+enum WsTag {
+    WS_NTT = 0,           // the NTT's inter-pass intermediate
+    WS_HOST_STAGING = 1,  // sa_ntt_host's device copies of host buffers
+    WS_PLAN_FLAG = 7,     // sa_interp_plan's zero flag
+    WS_TREE = 8,          // the subproduct tree of one call (poly_tree.cuh: tree_layout)
+    WS_INTERP_PLAN = 9,   // sa_interpolate's plan
+    WS_INTERP_APPLY = 10  // an apply's scratch
+};
+int get_workspace(void **out, size_t bytes, cudaStream_t st, WsTag tag);
 void keep_pool_memory();
 
 // ---------------------------------------------------------------- table cache --

@@ -3,8 +3,9 @@
 // barrier phase by barrier phase, so the index maps, twiddle tables and the
 // portable field arithmetic can be checked against the oracle without a GPU.
 // The host-side schedule around them (NTT plan and passes, Merkle launch loop,
-// fold scalars) is the library's own, from the same headers; only the launches
-// are replaced by CPU loops.
+// fold scalars, the subproduct tree's levels, walk, plan build and up-sweep) is
+// the library's own, from the same headers; only the launches are replaced by
+// CPU loops.
 // It is NOT a fallback: nothing in the product loads this library.
 //
 // Build: g++ -O2 -std=c++17 -shared -fPIC -o libsa_emu.so emu.cpp
@@ -19,6 +20,7 @@
 #include "../../stark-anatomy_b200/csrc/hash.cuh"
 #include "../../stark-anatomy_b200/csrc/ntt_plan.cuh"
 #include "../../stark-anatomy_b200/csrc/ntt_tile.cuh"
+#include "../../stark-anatomy_b200/csrc/poly_tree.cuh"
 
 using namespace sa;
 
@@ -153,6 +155,126 @@ int emu_ntt_ex(uint64_t *out, const uint64_t *in, int log_n, const uint64_t *roo
 }
 int emu_ntt(uint64_t *out, const uint64_t *in, int log_n, const uint64_t *root, int inverse, size_t batch) {
     return emu_ntt_ex(out, in, log_n, root, inverse, batch, 0);
+}
+
+}  // extern "C"
+
+// the backend of the subproduct tree's schedule (poly_tree.cuh): every kernel is a loop over its element function,
+// sa_ntt is emu_ntt, device memory is host memory
+struct EmuTree {
+    template <class F>
+    static int each(long long n, F f) {
+        for (long long i = 0; i < n; i++) f(i);
+        return SA_OK;
+    }
+    int leaves(fe *v0, const fe *d, long long k, long long K) {
+        return each(K, [&](long long i) { tree_leaves_elem(v0, d, k, i); });
+    }
+    int pad(fe *dst, const fe *src, long long K, int mlog) {
+        return each(2 * K, [&](long long i) { tree_pad_elem(dst, src, mlog, i); });
+    }
+    int pairmul(fe *out, const fe *in, long long K, int mlog) {
+        return each(K, [&](long long i) { tree_pairmul_elem(out, in, mlog, i); });
+    }
+    int cross(fe *out, const fe *Pt, const fe *Vt, long long K, long long batch, int mlog) {
+        return each(batch * K, [&](long long i) { tree_cross_elem(out, Pt, Vt, K, mlog, i); });
+    }
+    int fix(fe *parent, const fe *add, long long K, long long batch, int mlog, long long k) {
+        return each(batch * K / 2, [&](long long i) { tree_fix_elem(parent, add, K, mlog, k, i); });
+    }
+    int derivative(fe *out, const fe *z, long long k) {
+        return each(k, [&](long long i) { derivative_elem(out, z, i); });
+    }
+    int qleaves(fe *P0, const fe *values, const fe *inv_m, long long k, int logK, long long batch) {
+        return each(batch << logK, [&](long long i) { tree_qleaves_elem(P0, values, inv_m, k, logK, i); });
+    }
+    int root(fe *out, const fe *root, long long k, long long K) {
+        return each(k + 1, [&](long long i) { tree_root_elem(out, root, K, i); });
+    }
+    int series_pad(fe *W, const fe *z, long long k, const fe *alpha, long long s) {
+        return each(8 * s, [&](long long i) { series_pad_elem(W, z, k, alpha, s, i); });
+    }
+    int series_step(fe *W, long long n4) {
+        return each(n4, [&](long long i) { series_step_elem(W, n4, i); });
+    }
+    int eval_top_pad(fe *W, const fe *f, long long nf, const fe *alpha, long long n, long long n2) {
+        return each(2 * n2, [&](long long i) { eval_top_pad_elem(W, f, nf, alpha, n, n2, i); });
+    }
+    int pointwise_mul(fe *out, const fe *a, const fe *b, long long n) {
+        return each(n, [&](long long i) { pointwise_mul_elem(out, a, b, i); });
+    }
+    int eval_root(fe *c, const fe *s, long long n, long long k, long long K) {
+        return each(K, [&](long long i) { eval_root_elem(c, s, n, k, i); });
+    }
+    int down(fe *O, const fe *chat, const fe *VT, long long K, int mlog) {
+        return each(2 * K, [&](long long i) { tree_down_elem(O, chat, VT, mlog, i); });
+    }
+    int down_fix(fe *next, const fe *O, const fe *cur, long long K, int mlog, long long k) {
+        return each(K, [&](long long i) { tree_down_fix_elem(next, O, cur, mlog, k, i); });
+    }
+    // one group of 8 consecutive elements per thread: the inverses do not depend on the grouping
+    int batch_inverse(fe *inv_m, const fe *b, long long n, int *flag) {
+        return each((n + 7) / 8, [&](long long g) {
+            batch_inverse_group(b, n, 8 * g, 1, flag, [&](long long i, const fe &x) { inv_m[i] = x; });
+        });
+    }
+    int horner(fe *out, const fe *coeffs, long long ncoef, const fe *points, long long npoints) {
+        return each(npoints, [&](long long j) { out[j] = poly_horner(coeffs, ncoef, points[j]); });
+    }
+    int ntt(fe *out, const fe *in, int log_n, const uint64_t root[2], int inverse, size_t batch) {
+        return emu_ntt((uint64_t *)out, (const uint64_t *)in, log_n, root, inverse, batch);
+    }
+    int copy(fe *dst, const fe *src, size_t n) {
+        memmove(dst, src, sizeof(fe) * n);
+        return SA_OK;
+    }
+    int copy2d(fe *dst, size_t dpitch, const fe *src, size_t spitch, size_t width, size_t rows) {
+        for (size_t r = 0; r < rows; r++) memmove(dst + r * dpitch, src + r * spitch, sizeof(fe) * width);
+        return SA_OK;
+    }
+    int store(fe *dst, const fe &v) {
+        *dst = v;
+        return SA_OK;
+    }
+};
+
+extern "C" {
+
+// the library's tree schedules over EmuTree, at any k >= 1 (the library takes its direct kernels at small k)
+int emu_zerofier(uint64_t *out, const uint64_t *domain, size_t k) {
+    Tree t = tree_layout(k, TREE_ZEROFIER, 0);
+    std::vector<fe> ws(t.elems);
+    t.ws = ws.data();
+    EmuTree b;
+    return tree_zerofier(b, t, (fe *)out, (const fe *)domain);
+}
+// sa_poly_eval_mode 2: the walk down the tree; ncoef >= 1
+int emu_poly_eval_walk(uint64_t *out, const uint64_t *coeffs, size_t ncoef, const uint64_t *points, size_t npoints) {
+    Tree t = tree_layout(npoints, TREE_EVAL, ncoef);
+    std::vector<fe> ws(t.elems);
+    t.ws = ws.data();
+    EmuTree b;
+    return tree_poly_eval(b, t, (fe *)out, (const fe *)coeffs, ncoef, (const fe *)points);
+}
+size_t emu_interp_plan_bytes(size_t k) { return sizeof(fe) * interp_plan_layout(k, true).elems; }
+// sa_interp_plan with the tree's layout; walk != 0: M'(d_i) by the walk down the tree, else by Horner
+int emu_interp_plan(uint64_t *plan, const uint64_t *domain, size_t k, int walk) {
+    const InterpPlan L = interp_plan_layout(k, true);
+    if (L.elems == 0) return SA_ESIZE;
+    Tree t = tree_layout(k, TREE_PLAN, walk ? k : 0);
+    std::vector<fe> ws(t.elems);
+    t.ws = ws.data();
+    int flag = 0;
+    EmuTree b;
+    const int rc = interp_plan_tree(b, t, (fe *)plan, L, (const fe *)domain, walk != 0, &flag);
+    return rc != SA_OK ? rc : flag ? SA_EDIVZERO : SA_OK;
+}
+int emu_interp_apply_batch(uint64_t *out, const uint64_t *plan, const uint64_t *values, size_t k, size_t batch) {
+    const InterpPlan L = interp_plan_layout(k, true);
+    if (L.elems == 0) return SA_ESIZE;
+    std::vector<fe> ws(4 * (size_t)L.K * std::min(batch, interp_batch_max(L)));
+    EmuTree b;
+    return interp_apply_tree(b, (fe *)out, (const fe *)plan, L, (const fe *)values, k, batch, ws.data());
 }
 
 uint32_t emu_decimal(uint8_t *buf40, const uint64_t *x) {
