@@ -180,6 +180,49 @@ int sa_interp_apply_batch(void *out, const void *plan, const void *values, size_
  * k > 2^20.  Host-only: no CUDA call.                                                         */
 size_t sa_interp_batch_max(size_t k);
 
+/* ---- code/ntt.py:137-176 fast_coset_divide, many numerators over one divisor, and ntt.py:132-135
+ * fast_coset_evaluate, many polynomials in one call ------------------------------------------------
+ * n = 2^log_n, log_n in [1, 26]; `root` a primitive n-th root of unity (checked like sa_ntt's, before
+ * any launch: SA_EROOTORDER / SA_ENOTPRIM).  With R_i = r(offset * root^i) and L_i = l(offset * root^i),
+ * i < n, a row of an apply is out[j] = U[j] * offset^-j, j < qlen, U = intt(L_i / R_i): the reference's
+ * fast_coset_divide at order n before its truncation.  So where n/2 <= max(deg l, deg r) < n (the
+ * reference keeps order n) out[0 .. deg l - deg r] are its coefficients, bit for bit, and a clean
+ * division with deg l < n gives the exact quotient followed by zeros.
+ * A coset division plan holds what depends on (divisor, offset, root, log_n) alone: offset^i, 1/R_i and
+ * offset^-i (i < n).  It is a device buffer the caller owns, of sa_coset_div_plan_bytes(log_n) bytes;
+ * its layout is internal and depends on log_n alone (48 MiB at 2^20, 3 GiB at 2^26).
+ * sa_coset_div_plan_bytes: 0 when log_n is outside 1..26.  Host-only: no CUDA call.                 */
+size_t sa_coset_div_plan_bytes(int log_n);
+/* Builds the plan of divisor[0..dlen) on the coset offset * <root>.  SA_ESIZE for dlen outside 1..n or
+ * log_n outside 1..26, SA_EDIVZERO for offset == 0 (both before any launch) and when some R_i == 0 (the
+ * zero divisor among them: the reference's element-wise division raises there).  Synchronises (it
+ * reads the zero flag).                                                                          */
+int sa_coset_div_plan(void *plan, const void *divisor, size_t dlen, int log_n, const uint64_t root[2],
+                      const uint64_t offset[2], void *stream);
+/* out[b*qlen .. b*qlen+qlen) = row b of the division of lhs[b*ncoef .. b*ncoef+ncoef) by the plan's
+ * divisor, b < batch; log_n and root must be the plan's.  Rows are contiguous; out must not overlap
+ * lhs.  1 <= ncoef, qlen <= n, else SA_ESIZE before any launch; batch == 0 returns SA_OK without a
+ * launch.  Asynchronous: no host synchronisation, and no allocation once the stream's workspaces
+ * have grown for this log_n and chunk size, so the call can be captured in a CUDA graph after one
+ * call on the capturing stream (the graph keeps that stream's workspace: replay it where that
+ * stream's other work cannot run concurrently, and make no larger call on that stream while the
+ * graph is in use).  Reads the plan only: one plan may be applied on several streams at once.
+ * The batch runs in chunks of sa_coset_batch_max(log_n) rows; each chunk issues the same launches
+ * whatever its size (load, one batched forward sa_ntt, quotient, one batched inverse sa_ntt, store)
+ * and takes 32 bytes of per-stream workspace per element per row.                              */
+int sa_coset_div_apply_batch(void *out, const void *plan, const void *lhs, size_t ncoef, size_t qlen, int log_n,
+                             const uint64_t root[2], size_t batch, void *stream);
+/* out[b*n .. b*n+n) = fast_coset_evaluate of coeffs[b*ncoef .. b*ncoef+ncoef) at order n:
+ * ntt(coeffs[i] * offset^i, zero padded to n), b < batch.  Needs no plan.  The same checks (1 <=
+ * ncoef <= n), chunks and asynchronous promises as sa_coset_div_apply_batch; out must not overlap
+ * coeffs.                                                                                        */
+int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log_n, const uint64_t root[2],
+                            const uint64_t offset[2], size_t batch, void *stream);
+/* The most rows one chunk of sa_coset_div_apply_batch / sa_coset_evaluate_batch takes:
+ * max(1, floor(2^30 / (32 n))) (32 at 2^20, 512 at 2^16), so a chunk's workspace stays at or below
+ * 1 GiB; 0 when log_n is outside 1..26.  Host-only: no CUDA call.                                */
+size_t sa_coset_batch_max(int log_n);
+
 /* ---- code/merkle.py:6-14 Merkle.commit -------------------------------------------------
  * Builds the whole blake2b-512 tree over n = 2^k leaves, leaf = H(decimal ASCII of the
  * value), node = H(left || right).  `tree` receives 2n nodes of 64 bytes in heap order:

@@ -83,15 +83,18 @@ struct NttPlan : DeviceTables, NttTables {
 };
 using PlanPtr = std::shared_ptr<NttPlan>;
 
+int launch_pow_table(fe *out, const fe &base_m, const fe &lead_m, long long count, cudaStream_t st, int swz) {
+    const long long threads = (count + 15) / 16;
+    const int bs = 128;
+    k_pow_table<<<(unsigned)((threads + bs - 1) / bs), bs, 0, st>>>(out, base_m, lead_m, count, swz);
+    SA_LAUNCH_CHECK();
+    return SA_OK;
+}
 int build_pow_table(DeviceTables &owner, fe **out, const fe &base_m, const fe &lead_m, long long count,
                     cudaStream_t st, int swz) {
     int rc = owner.alloc((void **)out, sizeof(fe) * (size_t)count);
     if (rc != SA_OK) return rc;
-    const long long threads = (count + 15) / 16;
-    const int bs = 128;
-    k_pow_table<<<(unsigned)((threads + bs - 1) / bs), bs, 0, st>>>(*out, base_m, lead_m, count, swz);
-    SA_LAUNCH_CHECK();
-    return SA_OK;
+    return launch_pow_table(*out, base_m, lead_m, count, st, swz);
 }
 
 // validates the root like ntt.py:10-11 and returns (creating if needed) the plan.  Tables are built

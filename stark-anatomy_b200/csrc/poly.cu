@@ -1,10 +1,12 @@
 // poly.cu -- polynomial kernels: element-wise products and quotients, scaling, Horner evaluation, the
-// direct zerofier and Lagrange kernels, and the kernels of the subproduct tree (poly_tree.cuh) behind
-// sa_zerofier, sa_interpolate and sa_poly_eval, with the backend that launches them for the tree's schedule.
+// direct zerofier and Lagrange kernels, the kernels of the subproduct tree (poly_tree.cuh) behind
+// sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans and batched coset
+// evaluation (coset.cuh), with the backend that launches them for the headers' schedules.
 //
-// Reference behaviour reproduced (bit-exact): code/ntt.py:61-172, code/algebra.py:53-57,75-94.
+// Reference behaviour reproduced (bit-exact): code/ntt.py:61-176, code/algebra.py:53-57,75-94.
 #include <algorithm>
 
+#include "coset.cuh"
 #include "ntt_tile.cuh"
 #include "poly_tree.cuh"
 #include "runtime.cuh"
@@ -215,6 +217,17 @@ __global__ void k_tree_down_fix(fe *next, const fe *O, const fe *cur, long long 
     grid_stride(K, [&](long long idx) { tree_down_fix_elem(next, O, cur, mlog, k, idx); });
 }
 
+// ---- coset division and evaluation kernels: each runs its element function of coset.cuh over batch rows of n ----
+__global__ void k_coset_load(fe *ws, const fe *lhs, const fe *pw_m, long long ncoef, int log_n, long long batch) {
+    grid_stride(batch << log_n, [&](long long idx) { coset_load_elem(ws, lhs, pw_m, ncoef, log_n, idx); });
+}
+__global__ void k_coset_quot(fe *ws, const fe *inv_m, int log_n, long long batch) {
+    grid_stride(batch << log_n, [&](long long idx) { coset_quot_elem(ws, inv_m, log_n, idx); });
+}
+__global__ void k_coset_store(fe *out, const fe *ws, const fe *ipw_m, long long qlen, int log_n, long long batch) {
+    grid_stride(batch << log_n, [&](long long idx) { coset_store_elem(out, ws, ipw_m, qlen, log_n, idx); });
+}
+
 extern "C" {
 
 int sa_pointwise_mul(void *out, const void *a, const void *b, size_t n, void *stream) {
@@ -265,7 +278,8 @@ static int poly_eval_horner(void *out, const void *coeffs, size_t ncoef, const v
 
 }  // extern "C"
 
-// ---- the tree schedule's backend (poly_tree.cuh): its kernels, sa_ntt and the copies, on one stream ----
+// ---- the backend of the tree's and the coset schedules (poly_tree.cuh, coset.cuh): their kernels, sa_ntt and the
+// copies, on one stream ----
 static inline unsigned tree_grid(long long n) { return grid_for(n, 256, 8); }
 static inline unsigned blocks256(long long n) { return (unsigned)((n + 255) / 256); }
 // one method per kernel, launching it with its grid; the arguments are the kernel's
@@ -311,6 +325,14 @@ struct DeviceTree {
         return go<128>(k_batch_inverse, grid_for((n + 7) / 8, 128), im, b, n, flag);
     }
     int horner(fe *o, const fe *c, ll nc, const fe *x, ll nx) { return poly_eval_horner(o, c, nc, x, nx, st); }
+    int pow_table(fe *o, const fe &base_m, ll count) { return launch_pow_table(o, base_m, fe_mont_one(), count, st); }
+    int coset_load(fe *ws, const fe *l, const fe *pw, ll nc, int lg, ll nb) {
+        return go(k_coset_load, tree_grid(nb << lg), ws, l, pw, nc, lg, nb);
+    }
+    int coset_quot(fe *ws, const fe *inv, int lg, ll nb) { return go(k_coset_quot, tree_grid(nb << lg), ws, inv, lg, nb); }
+    int coset_store(fe *o, const fe *ws, const fe *ipw, ll q, int lg, ll nb) {
+        return go(k_coset_store, tree_grid(nb << lg), o, ws, ipw, q, lg, nb);
+    }
     int ntt(fe *o, const fe *i, int lg, const uint64_t *r, int inv, size_t nb) { return sa_ntt(o, i, lg, r, inv, nb, st); }
     int copy(fe *dst, const fe *src, size_t n) {
         SA_CUDA(cudaMemcpyAsync(dst, src, sizeof(fe) * n, cudaMemcpyDeviceToDevice, st));
@@ -469,6 +491,54 @@ int sa_poly_eval_mode(void *out, const void *coeffs, size_t ncoef, const void *p
 }
 int sa_poly_eval(void *out, const void *coeffs, size_t ncoef, const void *points, size_t npoints, void *stream) {
     return sa_poly_eval_mode(out, coeffs, ncoef, points, npoints, 0, stream);
+}
+
+// ---- coset division plans and batched coset evaluation (coset.cuh) ----
+size_t sa_coset_div_plan_bytes(int log_n) { return sizeof(fe) * coset_div_plan_layout(log_n).elems; }
+
+size_t sa_coset_batch_max(int log_n) { return coset_batch_max(log_n); }
+
+// scratch: the divisor's codeword (n elements, WS_COSET) and the zero flag (WS_PLAN_FLAG)
+int sa_coset_div_plan(void *plan, const void *divisor, size_t dlen, int log_n, const uint64_t root[2],
+                      const uint64_t offset[2], void *stream) {
+    SA_TRY(coset_div_plan_check(log_n, dlen, root, offset));
+    cudaStream_t st = (cudaStream_t)stream;
+    int *flag = nullptr;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&flag, 16, st, WS_PLAN_FLAG));
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) << log_n, st, WS_COSET));
+    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+    DeviceTree b{st};
+    SA_TRY(coset_div_plan_build(b, (fe *)plan, (const fe *)divisor, dlen, log_n, root, offset, ws, flag));
+    int h = 0;
+    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SA_CUDA(cudaStreamSynchronize(st));
+    return h ? SA_EDIVZERO : SA_OK;
+}
+
+// Reads the plan only; its scratch is the stream's workspace (WS_COSET): n elements per row of a chunk.
+int sa_coset_div_apply_batch(void *out, const void *plan, const void *lhs, size_t ncoef, size_t qlen, int log_n,
+                             const uint64_t root[2], size_t batch, void *stream) {
+    SA_TRY(coset_check(log_n, ncoef, qlen, root));
+    if (batch == 0) return SA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *ws = nullptr;
+    const size_t chunk = std::min(batch, coset_batch_max(log_n));
+    SA_TRY(get_workspace((void **)&ws, (sizeof(fe) << log_n) * chunk, st, WS_COSET));
+    DeviceTree b{st};
+    return coset_div_apply(b, (fe *)out, (const fe *)plan, (const fe *)lhs, ncoef, qlen, log_n, root, batch, ws);
+}
+
+// scratch: offset^i for i < ncoef (WS_COSET); the rows are transformed in out
+int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log_n, const uint64_t root[2],
+                            const uint64_t offset[2], size_t batch, void *stream) {
+    SA_TRY(coset_check(log_n, ncoef, 1, root));
+    if (batch == 0) return SA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *pw = nullptr;
+    SA_TRY(get_workspace((void **)&pw, sizeof(fe) * ncoef, st, WS_COSET));
+    DeviceTree b{st};
+    return coset_evaluate(b, (fe *)out, (const fe *)coeffs, ncoef, log_n, root, offset, batch, pw);
 }
 
 }  // extern "C"

@@ -202,8 +202,6 @@ inline const uint64_t *tree_root_of_unity(int log) {
     return table[log];
 }
 
-inline size_t sec16(size_t elems) { return (elems + 15) & ~(size_t)15; }  // rounded to 256 bytes
-
 // The tree of one call over k points and its workspace ws (element offsets into it):
 //   levels ((log K + 1) * K: level j at + j * K, the root at level log K)
 //   | node transforms, on a 256-byte boundary: every level's (log K * 2K, level j at + j * 2K) where the walk reads

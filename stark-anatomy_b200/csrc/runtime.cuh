@@ -81,12 +81,13 @@ static inline unsigned grid_for(long long n, int bs, int per_sm = 16) {
 // takes a tag that it or its caller still holds; distinct tags nest: sa_interpolate holds WS_INTERP_PLAN across
 // the plan build (WS_PLAN_FLAG, WS_TREE) and the apply (WS_INTERP_APPLY), and every sa_ntt inside them takes WS_NTT.
 enum WsTag {
-    WS_NTT = 0,           // the NTT's inter-pass intermediate
-    WS_HOST_STAGING = 1,  // sa_ntt_host's device copies of host buffers
-    WS_PLAN_FLAG = 7,     // sa_interp_plan's zero flag
-    WS_TREE = 8,          // the subproduct tree of one call (poly_tree.cuh: tree_layout)
-    WS_INTERP_PLAN = 9,   // sa_interpolate's plan
-    WS_INTERP_APPLY = 10  // an apply's scratch
+    WS_NTT = 0,            // the NTT's inter-pass intermediate
+    WS_HOST_STAGING = 1,   // sa_ntt_host's device copies of host buffers
+    WS_PLAN_FLAG = 7,      // the zero flag of sa_interp_plan and sa_coset_div_plan
+    WS_TREE = 8,           // the subproduct tree of one call (poly_tree.cuh: tree_layout)
+    WS_INTERP_PLAN = 9,    // sa_interpolate's plan
+    WS_INTERP_APPLY = 10,  // an apply's scratch
+    WS_COSET = 11          // coset division and evaluation (coset.cuh): the transformed rows, or offset^i
 };
 int get_workspace(void **out, size_t bytes, cudaStream_t st, WsTag tag);
 void keep_pool_memory();
@@ -130,7 +131,10 @@ std::shared_ptr<T> cache_publish(const CacheKey &key, std::shared_ptr<T> made) {
 }
 
 // ------------------------------------------------------------------- NTT (ntt.cu) --
-// count powers base^e * lead (Montgomery form) into a new table of `owner`; swz != 0 stores them in tile_tw_slot order
+// count powers base^e * lead (Montgomery form) into `out` (k_pow_table); swz != 0 stores them in tile_tw_slot order
+int launch_pow_table(sa::fe *out, const sa::fe &base_m, const sa::fe &lead_m, long long count, cudaStream_t st,
+                     int swz = 0);
+// the same into a new table of `owner`
 int build_pow_table(DeviceTables &owner, sa::fe **out, const sa::fe &base_m, const sa::fe &lead_m, long long count,
                     cudaStream_t st, int swz = 0);
 // the transform proper; `peers` (npeer <= TILE_MAX_PEERS) are extra destinations of the LAST pass: the

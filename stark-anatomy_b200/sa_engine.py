@@ -61,6 +61,11 @@ SYMBOLS = [
     ("sa_interp_apply", _ci, [_vp, _vp, _vp, _sz, _vp]),
     ("sa_interp_apply_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _vp]),
     ("sa_interp_batch_max", _sz, [_sz]),
+    ("sa_coset_div_plan_bytes", _sz, [_ci]),
+    ("sa_coset_div_plan", _ci, [_vp, _vp, _sz, _ci, _u64p, _u64p, _vp]),
+    ("sa_coset_div_apply_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _ci, _u64p, _sz, _vp]),
+    ("sa_coset_evaluate_batch", _ci, [_vp, _vp, _sz, _ci, _u64p, _u64p, _sz, _vp]),
+    ("sa_coset_batch_max", _sz, [_ci]),
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
@@ -106,6 +111,18 @@ class InterpPlan:
     def __init__(self, plan, k):
         self.plan = plan
         self.k = k
+
+
+class CosetDivPlan:
+    """A coset division plan (CudaEngine.coset_div_plan): the device buffer sa_coset_div_plan filled (torch.uint8)
+    for one divisor on the coset offset * <root> of order 2^log_n, with the scalars every apply passes again"""
+    __slots__ = ("plan", "log_n", "root", "offset")
+
+    def __init__(self, plan, log_n, root, offset):
+        self.plan = plan
+        self.log_n = log_n
+        self.root = root
+        self.offset = offset
 
 
 class CudaEngine:
@@ -297,6 +314,58 @@ class CudaEngine:
         if batch:
             self._check(self.lib.sa_interp_apply_batch(out.data_ptr(), plan.plan.data_ptr(), values.data_ptr(), plan.k,
                                                        batch, self._stream()))
+        return out
+
+    @staticmethod
+    def _rows(vecs, n):
+        """the batch of a (ncoef, 2) or (B, ncoef, 2) tensor with 1 <= ncoef <= n; "unsupported size" otherwise (the
+        library cannot see the tensors' shape)"""
+        if vecs.dim() not in (2, 3) or vecs.shape[-1] != 2 or not 1 <= vecs.shape[-2] <= n:
+            raise SaError(SA_ERRORS[-6])
+        return vecs.shape[0] if vecs.dim() == 3 else 1
+
+    def coset_div_plan(self, divisor, log_n, root, offset):
+        """sa_coset_div_plan: what dividing by `divisor` (dlen, 2) on the coset offset * <root> of order 2^log_n needs
+        of the divisor alone, kept on the device for coset_div_apply (synchronises; "divide by zero" when the divisor
+        vanishes somewhere on the coset, the zero divisor and offset 0 included)"""
+        nbytes = self.lib.sa_coset_div_plan_bytes(log_n)
+        if nbytes == 0 or divisor.dim() != 2:
+            raise SaError(SA_ERRORS[-6])
+        self._rows(divisor, 1 << log_n)
+        divisor = divisor.contiguous()
+        plan = self.torch.empty(nbytes, dtype=self.torch.uint8, device=self.device)
+        self._check(self.lib.sa_coset_div_plan(plan.data_ptr(), divisor.data_ptr(), divisor.shape[0], log_n,
+                                               _limbs(root), _limbs(offset), self._stream()))
+        return CosetDivPlan(plan, log_n, int(root), int(offset))
+
+    def coset_div_apply(self, plan, lhs, qlen):
+        """sa_coset_div_apply_batch: the first qlen coefficients of U(X) * offset^-j, U = intt(L / R) on the plan's
+        coset, for one numerator (ncoef, 2) -> (qlen, 2) or a batch of them (B, ncoef, 2) -> (B, qlen, 2) in one
+        call; asynchronous, the plan is only read"""
+        n = 1 << plan.log_n
+        batch = self._rows(lhs, n)
+        if not 1 <= qlen <= n:
+            raise SaError(SA_ERRORS[-6])
+        lhs = lhs.contiguous()
+        out = self.torch.empty(tuple(lhs.shape[:-2]) + (qlen, 2), dtype=self.torch.int64, device=self.device)
+        if batch:
+            self._check(self.lib.sa_coset_div_apply_batch(out.data_ptr(), plan.plan.data_ptr(), lhs.data_ptr(),
+                                                          lhs.shape[-2], qlen, plan.log_n, _limbs(plan.root), batch,
+                                                          self._stream()))
+        return out
+
+    def coset_evaluate(self, coeffs, log_n, root, offset):
+        """sa_coset_evaluate_batch: fast_coset_evaluate at order 2^log_n of one polynomial (ncoef, 2) -> (n, 2) or of
+        a batch (B, ncoef, 2) -> (B, n, 2) in one call; asynchronous"""
+        if self.lib.sa_coset_batch_max(log_n) == 0:
+            raise SaError(SA_ERRORS[-6])
+        n = 1 << log_n
+        batch = self._rows(coeffs, n)
+        coeffs = coeffs.contiguous()
+        out = self.torch.empty(tuple(coeffs.shape[:-2]) + (n, 2), dtype=self.torch.int64, device=self.device)
+        if batch:
+            self._check(self.lib.sa_coset_evaluate_batch(out.data_ptr(), coeffs.data_ptr(), coeffs.shape[-2], log_n,
+                                                         _limbs(root), _limbs(offset), batch, self._stream()))
         return out
 
     # --------------------------------------------------------------- merkle
