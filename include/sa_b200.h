@@ -115,13 +115,9 @@ int sa_ntt_host(void *out_host, const void *in_host, int log_n, const uint64_t r
 void *sa_host_alloc(size_t bytes);
 int sa_host_free(void *p);
 
-/* ---- element-wise pieces of fast_multiply / fast_coset_divide / fast_coset_evaluate ---- */
+/* ---- the element-wise piece of fast_multiply ------------------------------------------ */
 /* code/ntt.py:61  out[i] = a[i] * b[i]                                                   */
 int sa_pointwise_mul(void *out, const void *a, const void *b, size_t n, void *stream);
-/* code/ntt.py:172 out[i] = a[i] / b[i]; SA_EDIVZERO if some b[i] == 0 (synchronises).    */
-int sa_pointwise_div(void *out, const void *a, const void *b, size_t n, void *stream);
-/* code/univariate.py:153-154 as used at ntt.py:133,159-160,176: out[i] = in[i] * factor^i */
-int sa_scale(void *out, const void *in, size_t n, const uint64_t factor[2], void *stream);
 /* code/univariate.py:130-136 at many points (fast_evaluate's values, ntt.py:82-100):
  * out[j] = sum_i coeffs[i] * points[j]^i                                                 */
 int sa_poly_eval(void *out, const void *coeffs, size_t ncoef, const void *points, size_t npoints,
@@ -182,7 +178,7 @@ size_t sa_interp_batch_max(size_t k);
 
 /* ---- code/ntt.py:137-176 fast_coset_divide, many numerators over one divisor, and ntt.py:132-135
  * fast_coset_evaluate, many polynomials in one call ------------------------------------------------
- * n = 2^log_n, log_n in [1, 26]; `root` a primitive n-th root of unity (checked like sa_ntt's, before
+ * n = 2^log_n, log_n in [1, 30]; `root` a primitive n-th root of unity (checked like sa_ntt's, before
  * any launch: SA_EROOTORDER / SA_ENOTPRIM).  With R_i = r(offset * root^i) and L_i = l(offset * root^i),
  * i < n, a row of an apply is out[j] = U[j] * offset^-j, j < qlen, U = intt(L_i / R_i): the reference's
  * fast_coset_divide at order n before its truncation.  So where n/2 <= max(deg l, deg r) < n (the
@@ -190,13 +186,14 @@ size_t sa_interp_batch_max(size_t k);
  * division with deg l < n gives the exact quotient followed by zeros.
  * A coset division plan holds what depends on (divisor, offset, root, log_n) alone: offset^i, 1/R_i and
  * offset^-i (i < n).  It is a device buffer the caller owns, of sa_coset_div_plan_bytes(log_n) bytes;
- * its layout is internal and depends on log_n alone (48 MiB at 2^20, 3 GiB at 2^26).
- * sa_coset_div_plan_bytes: 0 when log_n is outside 1..26.  Host-only: no CUDA call.                 */
+ * its layout is internal and depends on log_n alone (48 MiB at 2^20, 6 GiB at 2^27, 48 GiB at 2^30:
+ * with the operands and workspaces, the largest sizes do not fit on one 80 GB device).
+ * Offset 0 is allowed, as in the reference: its powers are 1, 0, 0, ... and its inverse is 0.
+ * sa_coset_div_plan_bytes: 0 when log_n is outside 1..30.  Host-only: no CUDA call.                 */
 size_t sa_coset_div_plan_bytes(int log_n);
 /* Builds the plan of divisor[0..dlen) on the coset offset * <root>.  SA_ESIZE for dlen outside 1..n or
- * log_n outside 1..26, SA_EDIVZERO for offset == 0 (both before any launch) and when some R_i == 0 (the
- * zero divisor among them: the reference's element-wise division raises there).  Synchronises (it
- * reads the zero flag).                                                                          */
+ * log_n outside 1..30 (before any launch), SA_EDIVZERO when some R_i == 0 (the zero divisor among
+ * them: the reference's element-wise division raises there).  Synchronises (it reads the zero flag). */
 int sa_coset_div_plan(void *plan, const void *divisor, size_t dlen, int log_n, const uint64_t root[2],
                       const uint64_t offset[2], void *stream);
 /* out[b*qlen .. b*qlen+qlen) = row b of the division of lhs[b*ncoef .. b*ncoef+ncoef) by the plan's
@@ -220,7 +217,7 @@ int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log
                             const uint64_t offset[2], size_t batch, void *stream);
 /* The most rows one chunk of sa_coset_div_apply_batch / sa_coset_evaluate_batch takes:
  * max(1, floor(2^30 / (32 n))) (32 at 2^20, 512 at 2^16), so a chunk's workspace stays at or below
- * 1 GiB; 0 when log_n is outside 1..26.  Host-only: no CUDA call.                                */
+ * 1 GiB; 0 when log_n is outside 1..30.  Host-only: no CUDA call.                                */
 size_t sa_coset_batch_max(int log_n);
 
 /* ---- code/merkle.py:6-14 Merkle.commit -------------------------------------------------

@@ -39,7 +39,9 @@ SA_HD void coset_store_elem(fe *out, const fe *ws, const fe *ipw_m, long long ql
 }
 
 // ---- host schedule ----
-constexpr int COSET_MAX_LOG = 26;  // a plan of 3 GiB; the transforms themselves go to 2^30
+// The transforms' range.  A plan is 48 n bytes (6 GiB at 2^27, 48 GiB at 2^30), so with the operands and the
+// workspaces the largest sizes do not fit on one 80 GB device.
+constexpr int COSET_MAX_LOG = NTT_MAX_LOG_N;
 
 // A plan is a device buffer of coset_div_plan_layout(log_n).elems elements, laid out by log_n alone; every section
 // starts on a 256-byte (16-element) boundary:  offset^i (n) | 1/R_i (n) | offset^-i (n), all in Montgomery form, so
@@ -79,15 +81,15 @@ inline int coset_check(int log_n, size_t ncoef, size_t qlen, const uint64_t root
     if (ncoef < 1 || ncoef > n || qlen < 1 || qlen > n) return SA_ESIZE;
     return ntt_check_root(fe_to_mont(fe_from_limbs(root)), log_n);
 }
-// a plan build's: a divisor of 1..n coefficients, and an offset != 0 (an apply multiplies by offset^-j)
-inline int coset_div_plan_check(int log_n, size_t dlen, const uint64_t root[2], const uint64_t offset[2]) {
-    SA_TRY(coset_check(log_n, dlen, 1, root));
-    return fe_is_zero(fe_from_limbs(offset)) ? SA_EDIVZERO : SA_OK;
+// a plan build's: a divisor of 1..n coefficients.  Every offset is accepted, 0 included (see coset_div_plan_build).
+inline int coset_div_plan_check(int log_n, size_t dlen, const uint64_t root[2], const uint64_t * /*offset*/) {
+    return coset_check(log_n, dlen, 1, root);
 }
 
 // the plan of divisor[0..dlen) on the coset offset * <root>: the two power tables, then R = ntt(r_i * offset^i)
 // in ws (n elements) and its batch inversion into the plan.  Some R_i = 0 (the zero divisor among them) raises
-// *flag: the reference's l / r raises "divide by zero" there (algebra.py:92).
+// *flag: the reference's l / r raises "divide by zero" there (algebra.py:92).  Offset 0 is the reference's too:
+// its powers are 1, 0, 0, ... (scale keeps the constant term) and its inverse is 0 (algebra.py:87-89).
 template <class B>
 int coset_div_plan_build(B &b, fe *plan, const fe *divisor, size_t dlen, int log_n, const uint64_t root[2],
                          const uint64_t offset[2], fe *ws, int *flag) {

@@ -1,4 +1,4 @@
-// poly.cu -- polynomial kernels: element-wise products and quotients, scaling, Horner evaluation, the
+// poly.cu -- polynomial kernels: element-wise products, batch inversion, Horner evaluation, the
 // direct zerofier and Lagrange kernels, the kernels of the subproduct tree (poly_tree.cuh) behind
 // sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans and batched coset
 // evaluation (coset.cuh), with the backend that launches them for the headers' schedules.
@@ -24,31 +24,12 @@ __device__ __forceinline__ long long thread_index() { return (long long)blockIdx
 __global__ void k_pointwise_mul(fe *out, const fe *a, const fe *b, long long n) {
     grid_stride(n, [&](long long i) { pointwise_mul_elem(out, a, b, i); });
 }
-// batch_inverse_group over the grid: each thread takes groups of 8 elements `stride` apart
-template <class Emit>
-__device__ __forceinline__ void batch_inverse(const fe *b, long long n, int *zero_flag, Emit emit) {
+// inv_m[i] = Montgomery form of 1/b[i] (the interpolation plan's 1/M'(d_i), the coset plan's 1/R_i): each thread
+// runs batch_inverse_group on groups of 8 elements `stride` apart
+__global__ void k_batch_inverse(fe *inv_m, const fe *b, long long n, int *zero_flag) {
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long base = thread_index(); base < n; base += stride * 8)
-        batch_inverse_group(b, n, base, stride, zero_flag, emit);
-}
-// out = a / b
-__global__ void k_pointwise_div(fe *out, const fe *a, const fe *b, long long n, int *zero_flag) {
-    batch_inverse(b, n, zero_flag, [&](long long i, const fe &binv) { tile_st(out + i, fe_montmul(tile_ld(a + i), binv)); });
-}
-// inv_m[i] = Montgomery form of 1/b[i]: the interpolation plan's 1/M'(d_i)
-__global__ void k_batch_inverse(fe *inv_m, const fe *b, long long n, int *zero_flag) {
-    batch_inverse(b, n, zero_flag, [&](long long i, const fe &binv) { tile_st(inv_m + i, binv); });
-}
-// out[i] = in[i] * factor^i; thread handles i, i + T, i + 2T, ... with running factor^T
-__global__ void k_scale(fe *out, const fe *in, long long n, fe factor_m, fe factor_T_m) {
-    const long long T = (long long)gridDim.x * blockDim.x;
-    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    fe f = fe_mont_pow_u64(factor_m, (uint64_t)i);
-    for (; i < n; i += T) {
-        tile_st(out + i, fe_montmul(tile_ld(in + i), f));
-        f = fe_montmul(f, factor_T_m);
-    }
+        batch_inverse_group(b, n, base, stride, zero_flag, [&](long long i, const fe &binv) { tile_st(inv_m + i, binv); });
 }
 // Horner, one thread per point
 __global__ void k_poly_eval(fe *out, const fe *coeffs, long long ncoef, const fe *points, long long npts) {
@@ -234,34 +215,6 @@ int sa_pointwise_mul(void *out, const void *a, const void *b, size_t n, void *st
     if (n == 0) return SA_OK;
     k_pointwise_mul<<<grid_for((long long)n, 256), 256, 0, (cudaStream_t)stream>>>((fe *)out, (const fe *)a,
                                                                                    (const fe *)b, (long long)n);
-    SA_LAUNCH_CHECK();
-    return SA_OK;
-}
-
-int sa_pointwise_div(void *out, const void *a, const void *b, size_t n, void *stream) {
-    if (n == 0) return SA_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    int *flag = nullptr;
-    keep_pool_memory();
-    SA_CUDA(cudaMallocAsync((void **)&flag, sizeof(int), st));
-    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
-    k_pointwise_div<<<grid_for(((long long)n + 7) / 8, 128), 128, 0, st>>>((fe *)out, (const fe *)a,
-                                                                          (const fe *)b, (long long)n, flag);
-    SA_LAUNCH_CHECK();
-    int h = 0;
-    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    SA_CUDA(cudaStreamSynchronize(st));
-    cudaFreeAsync(flag, st);
-    return h ? SA_EDIVZERO : SA_OK;
-}
-
-int sa_scale(void *out, const void *in, size_t n, const uint64_t factor[2], void *stream) {
-    if (n == 0) return SA_OK;
-    const int bs = 256;
-    const unsigned grid = grid_for((long long)n, bs, 4);
-    const fe f_m = fe_to_mont(fe_from_limbs(factor));
-    const fe fT_m = fe_mont_pow_u64(f_m, (uint64_t)grid * bs);
-    k_scale<<<grid, bs, 0, (cudaStream_t)stream>>>((fe *)out, (const fe *)in, (long long)n, f_m, fT_m);
     SA_LAUNCH_CHECK();
     return SA_OK;
 }

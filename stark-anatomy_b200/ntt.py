@@ -4,8 +4,8 @@ Put this directory ahead of the reference's code/ directory on sys.path and
 ``from ntt import *`` (code/fast_stark.py:4, code/fri.py:4) resolves here.  Same
 names, signatures, value types (lists of ``algebra.FieldElement``,
 ``univariate.Polynomial``), assertion messages and list-length semantics as the
-reference; every transform, Hadamard product, coset scaling and element-wise
-division runs in the sm_90a kernels behind include/sa_b200.h.  No CPU fallback:
+reference; every transform, Hadamard product, coset evaluation and coset division
+runs in the sm_90a kernels behind include/sa_b200.h.  No CPU fallback:
 without the CUDA library the first call raises.
 
 Known divergence, in misuse only: when ``root_order`` is too small for the operands (degree >= root_order)
@@ -96,9 +96,8 @@ def _transform_length(ncoef, order):
     return total
 
 
-def _ntt_product(a, b, root, pointwise):
-    """ntt.py:52-64 on two zero-padded coefficient vectors: transform both, combine the codewords with
-    `pointwise` (eng.pointwise_mul / eng.pointwise_div), transform back"""
+def _ntt_product(a, b, root):
+    """ntt.py:52-64 on two zero-padded coefficient vectors: transform both, multiply the codewords, transform back"""
     eng = _engine()
     ln, rn = eng.length(a), eng.length(b)
     a = eng.ntt(a, _log2(ln), root)
@@ -107,8 +106,8 @@ def _ntt_product(a, b, root, pointwise):
         k = min(ln, rn)
         a, b = eng.slice(a, 0, k), eng.slice(b, 0, k)
         assert(k & (k - 1) == 0), "cannot compute intt of non-power-of-two sequence"
-    combined = pointwise(a, b)
-    return eng.ntt(combined, _log2(eng.length(combined)), root, inverse=True)
+    product = eng.pointwise_mul(a, b)
+    return eng.ntt(product, _log2(eng.length(product)), root, inverse=True)
 
 
 def fast_multiply(lhs, rhs, primitive_root, root_order):
@@ -127,7 +126,7 @@ def fast_multiply(lhs, rhs, primitive_root, root_order):
     rn = _transform_length(rhs_degree + 1, order)
     a = eng.pad(sa_devlist.to_device(lhs.coefficients[:lhs_degree + 1]), ln)
     b = eng.pad(sa_devlist.to_device(rhs.coefficients[:rhs_degree + 1]), rn)
-    product = _ntt_product(a, b, root, eng.pointwise_mul)
+    product = _ntt_product(a, b, root)
     return Polynomial(sa_devlist.from_device(eng.slice(product, 0, degree + 1), field))
 
 
@@ -204,9 +203,8 @@ def fast_coset_evaluate(polynomial, offset, generator, order):
     eng = _engine()
     if total <= 1:
         return polynomial.scale(offset).coefficients + [field.zero()] * (order - ncoef)
-    coeffs = sa_devlist.to_device(polynomial.coefficients)
-    scaled = eng.pad(eng.scale(coeffs, offset.value), total) if ncoef else eng.zeros(total)
-    return sa_devlist.wrap(eng.ntt(scaled, _log2(total), generator.value), field)
+    coeffs = sa_devlist.to_device(polynomial.coefficients) if ncoef else eng.zeros(1)
+    return sa_devlist.wrap(eng.coset_evaluate(coeffs, _log2(total), generator.value, offset.value), field)
 
 
 def fast_coset_divide(lhs, rhs, offset, primitive_root, root_order):  # clean division only!
@@ -224,10 +222,11 @@ def fast_coset_divide(lhs, rhs, offset, primitive_root, root_order):  # clean di
     root, order = _shrink(primitive_root.value, root_order, degree, field.p)
     eng = _engine()
     ln = _transform_length(lhs_degree + 1, order)
-    rn = _transform_length(rhs_degree + 1, order)
-    # scale(offset) then trim to degree+1 (ntt.py:159-166) == scale the trimmed coefficients
-    a = eng.pad(eng.scale(sa_devlist.to_device(lhs.coefficients[:lhs_degree + 1]), offset.value), ln)
-    b = eng.pad(eng.scale(sa_devlist.to_device(rhs.coefficients[:rhs_degree + 1]), offset.value), rn)
-    scaled_quotient = _ntt_product(a, b, root, eng.pointwise_div)  # raises "divide by zero" like algebra.py:92
-    kept = eng.slice(scaled_quotient, 0, lhs_degree - rhs_degree + 1)
-    return Polynomial(sa_devlist.from_device(eng.scale(kept, offset.inverse().value), field))
+    _transform_length(rhs_degree + 1, order)
+    # ntt.py:159-176 is the plan's apply at order ln, truncated to the quotient.  ln == order unless
+    # degree >= root_order; then the plan's root check raises what the reference's first ntt asserts.
+    numerator = sa_devlist.to_device(lhs.coefficients[:lhs_degree + 1])
+    divisor = sa_devlist.to_device(rhs.coefficients[:rhs_degree + 1])
+    plan = eng.coset_div_plan(divisor, _log2(ln), root, offset.value)  # raises "divide by zero" like algebra.py:92
+    quotient = eng.coset_div_apply(plan, numerator, lhs_degree - rhs_degree + 1)
+    return Polynomial(sa_devlist.from_device(quotient, field))

@@ -42,7 +42,7 @@ def device_mul(self, other):
     n = 1 << max((out_len - 1).bit_length(), 1)
     eng = sa_engine.get_engine()
     fa, fb = eng.pad(sa_devlist.to_device(a), n), eng.pad(sa_devlist.to_device(b), n)
-    prod = ntt._ntt_product(fa, fb, _root_of_unity(n), eng.pointwise_mul)
+    prod = ntt._ntt_product(fa, fb, _root_of_unity(n))
     return Polynomial(sa_devlist.from_device(eng.slice(prod, 0, out_len), a[0].field))
 
 

@@ -50,8 +50,6 @@ SYMBOLS = [
     ("sa_host_alloc", _vp, [_sz]),
     ("sa_host_free", _ci, [_vp]),
     ("sa_pointwise_mul", _ci, [_vp, _vp, _vp, _sz, _vp]),
-    ("sa_pointwise_div", _ci, [_vp, _vp, _vp, _sz, _vp]),
-    ("sa_scale", _ci, [_vp, _vp, _sz, _u64p, _vp]),
     ("sa_poly_eval", _ci, [_vp, _vp, _sz, _vp, _sz, _vp]),
     ("sa_poly_eval_mode", _ci, [_vp, _vp, _sz, _vp, _sz, _ci, _vp]),
     ("sa_zerofier", _ci, [_vp, _vp, _sz, _vp]),
@@ -257,18 +255,6 @@ class CudaEngine:
                                               b.contiguous().data_ptr(), a.shape[0], self._stream()))
         return out
 
-    def pointwise_div(self, a, b):
-        out = self.empty(a.shape[0])
-        self._check(self.lib.sa_pointwise_div(out.data_ptr(), a.contiguous().data_ptr(),
-                                              b.contiguous().data_ptr(), a.shape[0], self._stream()))
-        return out
-
-    def scale(self, vec, factor):
-        vec = vec.contiguous()
-        out = self.empty(vec.shape[0])
-        self._check(self.lib.sa_scale(out.data_ptr(), vec.data_ptr(), vec.shape[0], _limbs(factor), self._stream()))
-        return out
-
     def poly_eval(self, coeffs, points, mode=0):
         """values of the polynomial at the points; mode 0 = the library chooses, 1 = Horner kernel, 2 = walk down
         the subproduct tree of the points (sa_poly_eval_mode)"""
@@ -327,7 +313,7 @@ class CudaEngine:
     def coset_div_plan(self, divisor, log_n, root, offset):
         """sa_coset_div_plan: what dividing by `divisor` (dlen, 2) on the coset offset * <root> of order 2^log_n needs
         of the divisor alone, kept on the device for coset_div_apply (synchronises; "divide by zero" when the divisor
-        vanishes somewhere on the coset, the zero divisor and offset 0 included)"""
+        vanishes somewhere on the coset, the zero divisor included)"""
         nbytes = self.lib.sa_coset_div_plan_bytes(log_n)
         if nbytes == 0 or divisor.dim() != 2:
             raise SaError(SA_ERRORS[-6])

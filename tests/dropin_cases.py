@@ -18,6 +18,7 @@ from hostmirror_loader import load_host_types
 T = load_host_types()
 import ntt as N  # noqa: E402  (the drop-in, stark-anatomy_b200/ntt.py)
 import fri as F  # noqa: E402
+import oracle as O  # noqa: E402
 
 P = T.field.p
 
@@ -142,6 +143,23 @@ def case_poly_asserts():
     big = T.poly(range(1, 30))
     with pytest.raises(AssertionError, match="divide by zero"):
         N.fast_coset_divide(big * T.poly([1] * 9), zero_at_coset * T.poly([1] * 9), T.field.generator(), w, 64)
+    # misuse, degree >= root_order with a power-of-two length: the root check of the first order-32 transform
+    with pytest.raises(AssertionError, match="primitive root is not primitive nth root of unity, where n is len"):
+        N.fast_coset_divide(T.poly(range(1, 33)), T.poly(range(3, 13)), T.field.generator(),
+                            T.field.primitive_nth_root(16), 16)
+
+
+def case_coset_offset_zero():
+    """offset 0 is no error in the reference: scale(0) keeps the constant term and inverse(0) is 0, so a division of
+    degree >= 8 gives [l0 / r0, 0, ...] and raises only for r0 == 0, and an evaluation is l0 everywhere"""
+    n = 64
+    w, zero = T.field.primitive_nth_root(n), T.field.zero()
+    lhs, rhs = T.Polynomial(seeded(71, 30)), T.Polynomial(seeded(72, 12))
+    got = N.fast_coset_divide(lhs, rhs, zero, w, n)
+    assert vals(got.coefficients) == O.fast_coset_divide(vals(lhs.coefficients), vals(rhs.coefficients), 0, w.value, n)
+    assert vals(N.fast_coset_evaluate(lhs, zero, w, n)) == O.fast_coset_evaluate(vals(lhs.coefficients), 0, w.value, n)
+    with pytest.raises(AssertionError, match="divide by zero"):
+        N.fast_coset_divide(lhs, T.Polynomial([zero] + rhs.coefficients), zero, w, n)
 
 
 def case_fast_multiply_big(n):

@@ -10,7 +10,8 @@ engine is the CUDA one and has no fallback.
 import numpy as np
 
 import oracle as O
-from sa_engine import SA_ERRORS, SaError
+from coset_cases import formula
+from sa_engine import SA_ERRORS, CosetDivPlan, SaError
 
 
 class OracleEngine:
@@ -71,16 +72,53 @@ class OracleEngine:
         self._log("pointwise_mul", a.shape[0])
         return O.pointwise_mul_np(np.ascontiguousarray(a), np.ascontiguousarray(b))
 
-    def pointwise_div(self, a, b):
-        self._log("pointwise_div", a.shape[0])
-        try:
-            return O.pointwise_div_np(np.ascontiguousarray(a), np.ascontiguousarray(b))
-        except AssertionError:
-            raise SaError(SA_ERRORS[-4])
+    @staticmethod
+    def _coset_rows(vecs, n):
+        """CudaEngine._rows: the rows of a (ncoef, 2) or (B, ncoef, 2) array with 1 <= ncoef <= n"""
+        if vecs.ndim not in (2, 3) or vecs.shape[-1] != 2 or not 1 <= vecs.shape[-2] <= n:
+            raise SaError(SA_ERRORS[-6])
+        return vecs.reshape(-1, vecs.shape[-2], 2)
 
-    def scale(self, vec, factor):
-        self._log("scale", vec.shape[0])
-        return O.scale_np(vec, factor) if vec.shape[0] else vec
+    @staticmethod
+    def _oracle_ntt_check(fn, *args):
+        try:
+            return fn(*args)
+        except AssertionError as e:
+            raise SaError(str(e))
+
+    def coset_div_plan(self, divisor, log_n, root, offset):
+        self._log("coset_div_plan", divisor.shape[0], log_n)
+        if not 1 <= log_n <= 30 or divisor.ndim != 2:
+            raise SaError(SA_ERRORS[-6])
+        n = 1 << log_n
+        self._coset_rows(divisor, n)
+        scaled = np.zeros((n, 2), np.uint64)
+        scaled[:divisor.shape[0]] = O.scale_np(divisor, offset)
+        if not self._oracle_ntt_check(O.ntt_np, root, scaled).any(axis=1).all():
+            raise SaError(SA_ERRORS[-4])
+        return CosetDivPlan(O.from_np(divisor), log_n, root, offset)
+
+    def coset_div_apply(self, plan, lhs, qlen):
+        self._log("coset_div_apply", lhs.shape[-2], qlen)
+        n = 1 << plan.log_n
+        rows = self._coset_rows(lhs, n)
+        if not 1 <= qlen <= n:
+            raise SaError(SA_ERRORS[-6])
+        out = np.zeros((rows.shape[0], qlen, 2), np.uint64)
+        for b, row in enumerate(rows):
+            out[b] = O.to_np(formula(O.from_np(row), plan.plan, plan.offset, plan.root, n, qlen))
+        return out.reshape(lhs.shape[:-2] + (qlen, 2))
+
+    def coset_evaluate(self, coeffs, log_n, root, offset):
+        self._log("coset_evaluate", coeffs.shape[-2], log_n)
+        if not 1 <= log_n <= 30:
+            raise SaError(SA_ERRORS[-6])
+        n = 1 << log_n
+        rows = self._coset_rows(coeffs, n)
+        out = np.zeros((rows.shape[0], n, 2), np.uint64)
+        for b, row in enumerate(rows):
+            out[b] = O.to_np(self._oracle_ntt_check(O.fast_coset_evaluate, O.from_np(row), offset, root, n))
+        return out.reshape(coeffs.shape[:-2] + (n, 2))
 
     def poly_eval(self, coeffs, points):
         self._log("poly_eval", coeffs.shape[0], points.shape[0])

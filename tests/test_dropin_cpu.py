@@ -36,6 +36,10 @@ def test_poly_asserts():
     C.case_poly_asserts()
 
 
+def test_coset_offset_zero():
+    C.case_coset_offset_zero()
+
+
 def test_poly_split_recursion():
     C.case_poly_split_recursion()
 

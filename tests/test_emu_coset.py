@@ -9,7 +9,7 @@ import pytest
 
 import __graft_entry__ as G
 import oracle as O
-from coset_cases import Case, P, rand_poly
+from coset_cases import Case, P, formula, rand_poly
 
 SA_EROOTORDER, SA_ENOTPRIM, SA_EDIVZERO, SA_ESIZE = -2, -3, -4, -6
 _u64p = ctypes.c_void_p
@@ -84,20 +84,28 @@ def test_evaluate_matches_oracle(E, log_n, batch):
 
 
 @pytest.mark.parametrize("log_n", list(range(1, 11)))
-def test_divisors_that_vanish_on_the_coset(E, log_n):
-    """X - offset * root^3 vanishes at a coset point, the zero polynomial everywhere; offset 0 has no inverse"""
+def test_divisors_that_vanish_and_offset_zero(E, log_n):
+    """X - offset * root^3 vanishes at a coset point, the zero polynomial everywhere; on the coset of offset 0 every
+    R_i is r_0, so only a divisor with r_0 == 0 vanishes there, and an apply gives the formula's [l0 / r0, 0, ...]"""
     rng = random.Random(6000 + log_n)
     n = 1 << log_n
     root, offset = O.primitive_nth_root(n), rng.randrange(1, P)
     point = offset * pow(root, 3, P) % P
     assert plan(E, [P - point, 1], log_n, root, offset)[0] == SA_EDIVZERO
     assert plan(E, [0] * min(n, 3), log_n, root, offset)[0] == SA_EDIVZERO
-    assert plan(E, rand_poly(rng, min(n - 1, 2)), log_n, root, 0)[0] == SA_EDIVZERO
+    assert plan(E, [0, 1], log_n, root, 0)[0] == SA_EDIVZERO
     assert plan(E, rand_poly(rng, min(n - 1, 2)), log_n, root, offset)[0] == 0
+    d = [rng.randrange(1, P)] + rand_poly(rng, min(n - 1, 2))[1:]
+    rc, p = plan(E, d, log_n, root, 0)
+    assert rc == 0
+    lhs = rand_poly(rng, n - 1)
+    rc, out = apply(E, p, O.to_np(lhs)[None], n, log_n, root)
+    assert rc == 0
+    assert O.from_np(out[0]) == formula(lhs, d, 0, root, n, n) == [lhs[0] * O.inverse(d[0]) % P] + [0] * (n - 1)
 
 
 @pytest.mark.parametrize("log_n", [1, 2, 5, 10])
-def test_sizes_and_roots_are_checked(E, log_n):
+def test_sizes_outside_1_30_and_roots_are_checked(E, log_n):
     n = 1 << log_n
     root, offset = O.primitive_nth_root(n), 7
     d = rand_poly(random.Random(log_n), 0)
@@ -114,5 +122,5 @@ def test_sizes_and_roots_are_checked(E, log_n):
     assert apply(E, p, np.zeros((2, n + 1, 2), np.uint64), n, log_n, root)[0] == SA_ESIZE
     assert apply(E, p, lhs, n, log_n, O.primitive_nth_root(2 * n))[0] == SA_EROOTORDER
     assert apply(E, p, lhs[:0], n, log_n, root)[0] == 0
-    for bad in (0, 27):
+    for bad in (0, 31):
         assert plan(E, d, bad, root, offset)[0] == SA_ESIZE

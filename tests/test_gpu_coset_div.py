@@ -1,8 +1,8 @@
 """Coset division plans and batched coset evaluation on the device (sa_coset_div_plan, sa_coset_div_apply_batch and
-sa_coset_evaluate_batch through CudaEngine.coset_div_plan / coset_div_apply / coset_evaluate): every row against the
-oracle (tests/coset_cases.py) and against a single apply, large sizes against the one-shot engine route the drop-in's
-fast_coset_divide takes, batches across chunks, the launches of a chunk, errors before any launch, two streams
-sharing one plan and an apply captured in a CUDA graph."""
+sa_coset_evaluate_batch through CudaEngine.coset_div_plan / coset_div_apply / coset_evaluate, the route of the drop-in's
+fast_coset_divide and fast_coset_evaluate): every row against the oracle (tests/coset_cases.py) and against a single
+apply, large sizes by exact properties, batches across chunks, the launches of a chunk, errors before any launch, two
+streams sharing one plan and an apply captured in a CUDA graph."""
 import os
 import random
 import sys
@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import oracle as O
-from coset_cases import Case
+from coset_cases import Case, formula
 
 PKG = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "stark-anatomy_b200")
 if PKG not in sys.path:
@@ -77,16 +77,6 @@ def need_device(eng, log_n, batch, vectors=8):
         pytest.skip("2^%d, B = %d needs %.1f GiB free on the device, %.1f GiB are" % (log_n, batch, want / GIB, free / GIB))
 
 
-def oneshot(eng, lhs, rhs, offset, root, log_n, qlen):
-    """the device route of the drop-in's fast_coset_divide at order n, before its truncation: scale, pad, scale,
-    pad, two forward transforms, pointwise_div, inverse transform, scale by offset^-1"""
-    n = 1 << log_n
-    a = eng.pad(eng.scale(lhs, offset), n)
-    b = eng.pad(eng.scale(rhs, offset), n)
-    u = eng.ntt(eng.pointwise_div(eng.ntt(a, log_n, root), eng.ntt(b, log_n, root)), log_n, root, inverse=True)
-    return eng.scale(eng.slice(u, 0, qlen).contiguous(), O.inverse(offset))
-
-
 def cyclic_product(eng, a, b, log_n, root):
     """a * b at order n (exact when deg a + deg b < n)"""
     n = 1 << log_n
@@ -117,9 +107,10 @@ def test_apply_matches_oracle_and_single_applies(eng, log_n, batch, full):
 
 
 @pytest.mark.parametrize("log_n, batch", [(20, 3), (22, 3), (24, 1), (26, 1)])
-def test_large_sizes_match_the_oneshot_route(eng, log_n, batch):
-    """sizes the oracle cannot reach: every row equals the one-shot engine route on the same operands, and a clean
-    division q * r returns q followed by zeros"""
+def test_large_sizes_by_coset_property(eng, log_n, batch):
+    """sizes the oracle cannot reach: every row of n coefficients U * offset^-j evaluates on the coset to L / R
+    (coset_evaluate(out) * coset_evaluate(r) == coset_evaluate(lhs)), and a clean division q * r returns q followed
+    by zeros"""
     need_device(eng, log_n, batch + 1, vectors=10)
     n = 1 << log_n
     rng = random.Random(log_n)
@@ -129,10 +120,11 @@ def test_large_sizes_match_the_oneshot_route(eng, log_n, batch):
     lhs = rand_dev(eng, (batch, n), 20 + log_n)
     plan = eng.coset_div_plan(r, log_n, root, offset)
     out = eng.coset_div_apply(plan, lhs, n)
+    R = eng.coset_evaluate(r, log_n, root, offset)
     for b in range(batch):
-        want = oneshot(eng, lhs[b], r, offset, root, log_n, n)
-        assert bool((out[b] == want).all()), b
-    del lhs, out, want
+        got = eng.pointwise_mul(eng.coset_evaluate(out[b], log_n, root, offset), R)
+        assert bool((got == eng.coset_evaluate(lhs[b], log_n, root, offset)).all()), b
+    del lhs, out, got, R
     q = rand_dev(eng, (n - dr - 1,), 30 + log_n)
     clean = cyclic_product(eng, q, r, log_n, root)
     got = eng.coset_div_apply(plan, clean, n)
@@ -175,19 +167,23 @@ def test_a_chunk_launches_what_one_row_does(eng, log_n):
 
 
 @pytest.mark.parametrize("log_n", [3, 12])
-def test_divisors_that_vanish_on_the_coset(eng, log_n):
-    """a divisor with a zero on the coset (X - offset * root^3), the zero divisor and offset 0 raise "divide by zero"
-    at plan time"""
+def test_divisors_that_vanish_and_offset_zero(eng, log_n):
+    """a divisor with a zero on the coset (X - offset * root^3), the zero divisor and, on the coset of offset 0, a
+    divisor with r_0 == 0 raise "divide by zero" at plan time; offset 0 with r_0 != 0 gives the formula's row"""
     n = 1 << log_n
     root, offset = O.primitive_nth_root(n), 11
     point = offset * pow(root, 3, P) % P
-    for d, off in (([P - point, 1], offset), ([0, 0, 0], offset), ([1, 2, 3], 0)):
+    for d, off in (([P - point, 1], offset), ([0, 0, 0], offset), ([0, 2, 3], 0)):
         with pytest.raises(AssertionError, match="divide by zero"):
             eng.coset_div_plan(up(eng, O.to_np(d)), log_n, root, off)
+    lhs = [random.Random(log_n).randrange(P) for _ in range(n)]
+    plan = eng.coset_div_plan(up(eng, O.to_np([1, 2, 3])), log_n, root, 0)
+    got = O.from_np(down(eng.coset_div_apply(plan, up(eng, O.to_np(lhs)), n)))
+    assert got == formula(lhs, [1, 2, 3], 0, root, n, n) == [lhs[0]] + [0] * (n - 1)
 
 
 @pytest.mark.parametrize("log_n", [3, 12])
-def test_bad_roots_and_sizes_are_refused_before_any_launch(eng, log_n):
+def test_bad_roots_and_sizes_outside_1_30_are_refused_before_any_launch(eng, log_n):
     import torch
     n = 1 << log_n
     root = O.primitive_nth_root(n)
@@ -215,7 +211,7 @@ def test_bad_roots_and_sizes_are_refused_before_any_launch(eng, log_n):
         with pytest.raises(AssertionError, match="unsupported size"):
             eng.coset_div_apply(plan, lhs, qlen)
     for divisor, lg in ((torch.zeros((n + 1, 2), dtype=torch.int64, device=eng.device), log_n),
-                        (torch.zeros((0, 2), dtype=torch.int64, device=eng.device), log_n), (d, 0), (d, 27)):
+                        (torch.zeros((0, 2), dtype=torch.int64, device=eng.device), log_n), (d, 0), (d, 31)):
         with pytest.raises(AssertionError, match="unsupported size"):
             eng.coset_div_plan(divisor, lg, root, 7)
     out = eng.coset_div_apply(plan, lhs[:0], n // 2)
@@ -288,14 +284,37 @@ def test_evaluate_matches_oracle(eng, log_n, batch):
         assert tuple(one.shape) == (n, 2) and (down(one) == got[0]).all()
 
 
-def test_evaluate_2_20_matches_the_engine_route(eng):
-    """at 2^20, every row equals the drop-in's fast_coset_evaluate route on the engine: scale, pad, ntt"""
+def test_evaluate_2_20_matches_oracle(eng):
+    """at 2^20, every row equals the oracle's fast_coset_evaluate"""
     log_n, batch = 20, 3
     need_device(eng, log_n, batch)
     n = 1 << log_n
     root, offset = O.primitive_nth_root(n), 85408008396924667383611388730472331217
     coeffs = rand_dev(eng, (batch, n // 4 + 3), 11)
-    out = eng.coset_evaluate(coeffs, log_n, root, offset)
-    for b in range(batch):
-        want = eng.ntt(eng.pad(eng.scale(coeffs[b], offset), n), log_n, root)
-        assert bool((out[b] == want).all()), b
+    got = down(eng.coset_evaluate(coeffs, log_n, root, offset))
+    for b, row in enumerate(down(coeffs)):
+        assert O.from_np(got[b]) == O.fast_coset_evaluate(O.from_np(row), offset, root, n), b
+
+
+@pytest.mark.parametrize("log_n", [27, 28])
+def test_sizes_past_2_26(eng, log_n):
+    """2^27 and 2^28: a clean division q * r returns q followed by zeros, and an evaluation equals Horner
+    (poly_eval) at sampled coset points"""
+    need_device(eng, log_n, 1, vectors=8)
+    n = 1 << log_n
+    rng = random.Random(log_n)
+    root, offset = O.primitive_nth_root(n), rng.randrange(1, P)
+    dr = n // 4
+    r = rand_dev(eng, (dr + 1,), 10 + log_n)
+    q = rand_dev(eng, (n - dr - 1,), 30 + log_n)
+    clean = cyclic_product(eng, q, r, log_n, root)
+    plan = eng.coset_div_plan(r, log_n, root, offset)
+    got = eng.coset_div_apply(plan, clean, n)
+    assert bool((got[:q.shape[0]] == q).all())
+    assert not bool(got[q.shape[0]:].any())
+    del clean, plan, got
+    f = q[:n // 64 + 3]  # Horner's work is coefficients x points
+    idx = sorted({0, 1, n // 2, n - 1} | {rng.randrange(n) for _ in range(60)})
+    points = up(eng, O.to_np([offset * pow(root, i, P) % P for i in idx]))
+    ev = eng.coset_evaluate(f, log_n, root, offset)
+    assert bool((ev[idx] == eng.poly_eval(f, points, mode=1)).all())

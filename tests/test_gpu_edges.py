@@ -103,16 +103,31 @@ def test_device_product_on_boundaries(eng, vectors):
         assert g == u * v % P, t
 
 
-def test_device_inverse_on_boundaries(eng, vectors):
-    """sa_pointwise_div(1, b) in calls of at most 128 elements: one CTA, one divisor per thread's batch
-    inversion, so each quotient is one fe_mont_inv of b"""
+def plan_sections(plan, n):
+    """the offset^i, 1/R_i and offset^-i sections of a coset division plan of n >= 16 elements (Montgomery form)"""
+    raw = plan.plan.cpu().numpy().view(np.uint64).reshape(3, n, 2)
+    return raw[0], raw[1], raw[2]
+
+
+def mont(x):
+    """the Montgomery form x * 2^128 mod p of uint64[n, 2]"""
+    return O.pointwise_mul_np(np.ascontiguousarray(x), np.tile(O._fe((1 << 128) % P), (x.shape[0], 1)))
+
+
+def test_batch_inverse_on_boundaries(eng, vectors):
+    """k_batch_inverse through a coset division plan of order 128 and offset 1 whose divisor is the inverse transform
+    of the chosen values, so R_i are those values: one CTA, one divisor per thread's batch inversion, so each entry
+    of the plan's 1/R_i section is one fe_mont_inv of a chosen value"""
     muls, _, invs, _ = vectors
     divisors = invs + [b for _, b, _ in muls[::8] if b]
-    for lo in range(0, len(divisors), 128):
-        chunk = divisors[lo:lo + 128]
-        ones = O.to_np([1] * len(chunk))
-        got = O.from_np(down(eng, eng.pointwise_div(up(eng, ones), up(eng, O.to_np(chunk)))))
-        assert got == [pow(v, P - 2, P) for v in chunk]
+    n = 128
+    root = O.primitive_nth_root(n)
+    for lo in range(0, len(divisors), n):
+        chunk = divisors[lo:lo + n]
+        values = chunk + [1] * (n - len(chunk))
+        plan = eng.coset_div_plan(up(eng, O.to_np(O.intt(root, values))), 7, root, 1)
+        inv = O.from_np(plan_sections(plan, n)[1])
+        assert [v * RINV % P for v in inv[:len(chunk)]] == [pow(v, P - 2, P) for v in chunk]
 
 
 # ---- grid-stride kernels past their first sweep ----------------------------------------------------------
@@ -128,16 +143,25 @@ def _element_of_order_dividing(T):
     raise AssertionError("no element of order %d" % g)
 
 
-def test_scale_past_wrap(eng, sms):
-    """k_scale: thread i starts at factor^i and steps by the host's factor^T (T = 4 * SMs * 256)"""
-    T = 4 * sms * 256
-    n = past_wrap(T)
+def test_coset_powers_past_wrap(eng, sms):
+    """k_coset_load loops past its 8 * SMs * 256 threads: the plan's offset^i and offset^-i
+    tables (k_pow_table) equal the oracle's powers, and an evaluation row equals the oracle's fast_coset_evaluate,
+    for offsets 0, 1, p - 1, a random one and one whose powers repeat with the load's sweep T"""
+    T = 8 * sms * 256
+    log_n = T.bit_length()
+    n = 1 << log_n
+    root = O.primitive_nth_root(n)
     x = rand_np(8100, n)
     x[T] = O._fe(P - 1)
     vx = up(eng, x)
+    ones = O.to_np([1] * n)
     rng = random.Random(8101)
     for f in (0, 1, P - 1, rng.randrange(2, P), _element_of_order_dividing(T)):
-        assert (down(eng, eng.scale(vx, f)) == O.scale_np(x, f)).all(), f
+        pw, _, ipw = plan_sections(eng.coset_div_plan(up(eng, O.to_np([1])), log_n, root, f), n)
+        assert (pw == mont(O.scale_np(ones, f))).all(), f
+        assert (ipw == mont(O.scale_np(ones, O.inverse(f)))).all(), f
+        got = O.from_np(down(eng, eng.coset_evaluate(vx, log_n, root, f)))
+        assert got == O.fast_coset_evaluate(O.from_np(x), f, root, n), f
 
 
 def test_pointwise_mul_past_wrap(eng, sms):
@@ -147,27 +171,24 @@ def test_pointwise_mul_past_wrap(eng, sms):
     assert (down(eng, eng.pointwise_mul(up(eng, a), up(eng, b))) == O.pointwise_mul_np(a, b)).all()
 
 
-def test_pointwise_div_past_wrap(eng, sms):
-    """k_pointwise_div: one sweep is 16 * SMs CTAs of 128 threads, each inverting 8 strided divisors at once.
-    The quotient is checked exactly (q * b == a elementwise) and against the oracle on a sample; a zero
-    divisor in the second sweep or in the ragged tail must be reported."""
+def test_batch_inverse_past_wrap(eng, sms):
+    """k_batch_inverse: one sweep is 16 * SMs CTAs of 128 threads, each inverting
+    8 strided elements at once.  A coset plan just past one sweep holds 1/R_i with inv_i * R_i == 2^128 at every i
+    (R from an evaluation of the divisor); a divisor vanishing at one coset point in the second sweep or in the
+    last 8 must be reported."""
+    import torch
     S = 16 * sms * 128 * 8
-    n = past_wrap(S)
-    a, b = rand_np(8300, n), rand_np(8301, n)
-    b[b.sum(axis=1) == 0] = 1
-    a[S] = O._fe(P - 1)
-    b[S + 1] = O._fe(P - 1)
-    va, vb = up(eng, a), up(eng, b)
-    q = down(eng, eng.pointwise_div(va, vb))
-    assert (O.pointwise_mul_np(q, b) == a).all()
-    rng = random.Random(8302)
-    idx = sorted({0, S - 1, S, S + 1, 2 * S - 1, 2 * S, n - 1} | {rng.randrange(n) for _ in range(2000)})
-    assert (q[idx] == O.pointwise_div_np(a[idx], b[idx])).all()
-    for z in (S + 12345, n - 5):  # second sweep, ragged tail
-        bz = vb.clone()
-        bz[z] = 0
+    log_n = S.bit_length()
+    n = 1 << log_n
+    root, offset = O.primitive_nth_root(n), random.Random(8300).randrange(2, P)
+    divisor = up(eng, rand_np(8301, n))
+    inv = eng.coset_div_plan(divisor, log_n, root, offset).plan.view(torch.int64).reshape(3, n, 2)[1]
+    R = eng.coset_evaluate(divisor, log_n, root, offset)
+    assert (down(eng, eng.pointwise_mul(inv, R)) == O._fe((1 << 128) % P)).all()
+    for z in (S + 12345, n - 5):  # second sweep, last group of 8
+        vanishing = up(eng, O.to_np([P - offset * pow(root, z, P) % P, 1]))
         with pytest.raises(AssertionError, match="divide by zero"):
-            eng.pointwise_div(va, bz)
+            eng.coset_div_plan(vanishing, log_n, root, offset)
 
 
 @pytest.mark.parametrize("log_n", [20, 21])
