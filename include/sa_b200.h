@@ -224,15 +224,37 @@ size_t sa_coset_batch_max(int log_n);
  * Builds the whole blake2b-512 tree over n = 2^k leaves, leaf = H(decimal ASCII of the
  * value), node = H(left || right).  `tree` receives 2n nodes of 64 bytes in heap order:
  * node 1 is the root, node i has children 2i and 2i+1, leaf j is node n + j, node 0 is
- * unused.                                                                                 */
+ * unused (set to zero).  It is sa_merkle_tree_batch with batch 1.                          */
 int sa_merkle_tree(void *tree, const void *values, size_t n, void *stream);
+/* The trees of `batch` codewords of n leaves each, in one launch ladder: tree b (2n nodes of
+ * 64 bytes, sa_merkle_tree's layout) at trees + b*2n*64 bytes, built from values[b*n .. b*n+n).
+ * A batch issues exactly the launches of one tree of n leaves, up to 65535 trees; larger
+ * batches run in groups of 65535.  n not a power of two gives SA_ENOTPOW2 and batch == 0
+ * returns SA_OK, both without a launch.  Asynchronous; a call with more trees than any
+ * earlier call on the stream synchronises the stream once to grow its arrival counters.    */
+int sa_merkle_tree_batch(void *trees, const void *values, size_t n, size_t batch, void *stream);
 /* code/merkle.py:16-27 Merkle.open for k leaf indices (HOST array): paths_out receives
- * k * log2(n) digests of 64 bytes, siblings bottom-up per index (device memory).          */
+ * k * log2(n) digests of 64 bytes, siblings bottom-up per index (device memory).  It is
+ * sa_merkle_open_batch with batch 1.                                                      */
 int sa_merkle_open(void *paths_out, const void *tree, size_t n, const uint64_t *indices_host, size_t k,
                    void *stream);
-/* out[i] = values[indices[i]] (the leaf triples of code/fri.py:104-105).                  */
+/* The same k leaf indices opened in each of `batch` trees laid out as sa_merkle_tree_batch
+ * lays them: paths_out[b][q][level] = the sibling at `level` (bottom-up) of leaf indices[q]
+ * in tree b, 64 bytes each.  One index upload, one launch.  Before any launch: SA_ENOTPOW2
+ * for n not a power of two, SA_EINDEX for any index >= n; batch == 0, k == 0 or n == 1
+ * (no siblings) returns SA_OK without a launch.  Asynchronous.                            */
+int sa_merkle_open_batch(void *paths_out, const void *trees, size_t n, size_t batch, const uint64_t *indices_host,
+                         size_t k, void *stream);
+/* out[i] = values[indices[i]] (the leaf triples of code/fri.py:104-105).  It is
+ * sa_gather_batch with batch 1.                                                           */
 int sa_gather(void *out, const void *values, size_t n, const uint64_t *indices_host, size_t k,
               void *stream);
+/* out[b*k + q] = values[b*n + indices[q]]: the same k indices gathered from each of `batch`
+ * rows of n elements (any n >= 1), one index upload, one launch.  SA_EINDEX for any index
+ * >= n before any launch; batch == 0 or k == 0 returns SA_OK without a launch.
+ * Asynchronous.                                                                           */
+int sa_gather_batch(void *out, const void *values, size_t n, size_t batch, const uint64_t *indices_host, size_t k,
+                    void *stream);
 
 /* ---- code/fri.py:85 split-and-fold, and the fused round of Fri.commit (fri.py:64-88) ----
  * next[i] = 2^-1 * ((1 + alpha/(offset*omega^i)) * cw[i] + (1 - alpha/(offset*omega^i)) * cw[n/2+i])

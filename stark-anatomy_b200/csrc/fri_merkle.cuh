@@ -12,6 +12,7 @@ namespace sa {
 
 constexpr int MK_THREADS = 256;  // threads per Merkle CTA
 constexpr int MK_MAX_IPT_LOG = 3;  // a thread reduces at most 8 bottom nodes privately
+constexpr int MK_MAX_TREES = 65535;  // trees per launch: the tree of a CTA is blockIdx.y
 
 // c'[i] = 2^-1 (a + b) + (alpha * 2^-1 * x_i^-1) (a - b)   ==  fri.py:85
 //   inv2_m : 2^-1 in Montgomery form
@@ -32,7 +33,9 @@ SA_HD fe merkle_ld_stream(const fe *p) {
 }
 
 struct MerkleArgs {
-    uint64_t *tree;      // heap layout, 8 words per node
+    uint64_t *tree;      // heap layout, 8 words per node; tree b of a batch at tree + b * tree_stride
+    long long tree_stride;  // words from one tree of a batch to the next (16 per leaf), 0 without a batch
+    long long row_stride;   // mode 1: elements from one codeword row of a batch to the next
     long long width;     // number of bottom nodes of this launch
     int chunk;           // bottom nodes per CTA (power of two, <= MK_THREADS << ipt_log)
     int ipt_log;         // log2 of the bottom nodes one thread reduces privately (0..3)
@@ -46,11 +49,21 @@ struct MerkleArgs {
     const fe *xinv;      // mode 2: xinv[i] = omega^-i in Montgomery form, i < width
     fe s_m;              // mode 2: alpha * 2^-1 * offset^-1 in Montgomery form
     fe inv2_m;           // mode 2: 2^-1 in Montgomery form
-    unsigned int *ticket;  // optional: CTA arrival counter (zero between launches); the CTA that arrives last
-                         // also reduces the gridDim.x (<= MK_THREADS) subtree roots, saving a launch
-    uint64_t *root_out;  // last launch of a tree, optional: host-mapped landing pad, receives the root
+    unsigned int *ticket;  // optional: CTA arrival counters, one per tree (zero between launches); the CTA of a
+                         // tree that arrives last also reduces its gridDim.x (<= MK_THREADS) subtree roots,
+                         // saving a launch
+    uint64_t *root_out;  // last launch of a single tree, optional: host-mapped landing pad, receives the root
     unsigned long long root_seq;  // (8 words) and then this sequence number in word 8
 };
+
+// the arguments of tree b of a batch: its nodes, its codeword row and its arrival counter
+SA_HD MerkleArgs merkle_view(const MerkleArgs &a, long long b) {
+    MerkleArgs v = a;
+    v.tree += b * a.tree_stride;
+    v.values += b * a.row_stride;
+    if (v.ticket) v.ticket += b;
+    return v;
+}
 
 // launch shape for a level of `width` bottom nodes: small levels are latency bound (one node per
 // thread, 64..256-node CTAs so that 128-256 CTAs are in flight, each reducing its chunk to one digest); big ones are
@@ -111,8 +124,8 @@ inline void merkle_shape_override(MerkleArgs &a, const char *spec) {
     }
 }
 
-// Launches of one tree: the first handles the bottom level in a.mode, later ones continue from the
-// digests the previous one left.  With an arrival counter (`ticket`), the launch that leaves at most
+// Launches of one tree: the first handles the bottom level in a.mode (and, in mode 1, zeroes the unused
+// node 0), later ones continue from the digests the previous one left.  With an arrival counter (`ticket`), the launch that leaves at most
 // MK_THREADS single-digest CTAs also reduces those; without one, that takes one more launch.
 // shape_spec (nullptr: none) goes to merkle_shape_override.  launch(a, last) runs one launch and returns
 // 0 or an error code; `last` marks the launch that finishes the tree.
@@ -130,6 +143,21 @@ int merkle_launches(MerkleArgs a, unsigned int *ticket, const char *shape_spec, 
         a.width = left;
         a.mode = 0;
     }
+}
+
+// Launches of `batch` trees of one width (merkle_view lays them out): groups of up to MK_MAX_TREES trees,
+// each group issuing the launches of one tree.  tickets(trees) returns the arrival counters of a group
+// (nullptr: none); launch(a, trees, last) runs one launch over the group's trees.
+template <class Tickets, class Launch>
+int merkle_batch_launches(const MerkleArgs &a, long long batch, Tickets &&tickets, const char *shape_spec,
+                          Launch &&launch) {
+    for (long long b0 = 0; b0 < batch; b0 += MK_MAX_TREES) {
+        const int trees = (int)(batch - b0 < MK_MAX_TREES ? batch - b0 : MK_MAX_TREES);
+        const int rc = merkle_launches(merkle_view(a, b0), tickets(trees), shape_spec,
+                                       [&](MerkleArgs &m, bool last) { return launch(m, trees, last); });
+        if (rc != 0) return rc;
+    }
+    return 0;
 }
 
 // the scalars of a fold (fri.py:85) in Montgomery form: inv2_m = 2^-1, s_m = alpha * 2^-1 * offset^-1.

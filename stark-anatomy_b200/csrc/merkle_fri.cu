@@ -43,11 +43,16 @@ __device__ __forceinline__ void merkle_publish_root(const MerkleArgs &a, const u
 // fold -> leaf digest -> subtree, one pass over the codeword.
 // The 2 in __launch_bounds__ is the minimum of resident CTAs per SM, i.e. at most 128 registers: without
 // the bound the kernel drifts above 128 registers and only one CTA fits per SM.
-__global__ void __launch_bounds__(MK_THREADS, 2) k_merkle_chunk(const __grid_constant__ MerkleArgs a) {
+// A batch of trees of one width is one launch: blockIdx.y is the tree, so gridDim.x stays the CTA count
+// of one tree and the launch shape, the fused top's arrival count and the heap indices are those of a
+// single tree.
+__global__ void __launch_bounds__(MK_THREADS, 2) k_merkle_chunk(const __grid_constant__ MerkleArgs args) {
     __shared__ uint64_t sm[MK_THREADS * 8];
+    const MerkleArgs a = merkle_view(args, blockIdx.y);
     const long long blk = blockIdx.x;
     const unsigned nblocks = gridDim.x;
     const int tid = threadIdx.x;
+    if (a.mode == 1 && blk == 0 && tid < 8) a.tree[tid] = 0;  // the unused node 0
     const int active = a.chunk >> a.ipt_log;  // threads with a private subtree
     uint64_t d[8];
     if (tid < active) merkle_private(d, a, blk, tid);
@@ -95,9 +100,9 @@ __global__ void __launch_bounds__(MK_THREADS, 2) k_merkle_chunk(const __grid_con
             __syncthreads();
         }
         if (pass == 1 || a.ticket == nullptr) break;
-        // Every CTA has reduced its chunk to one digest (heap node nblocks + blk).  The CTA that
-        // arrives last reduces those nblocks digests as well instead of leaving them to one more
-        // launch (each thread fences its own stores, the barrier orders them before the ticket).
+        // Every CTA of this tree has reduced its chunk to one digest (heap node nblocks + blk).  The
+        // CTA that arrives last reduces those nblocks digests as well instead of leaving them to one
+        // more launch (each thread fences its own stores, the barrier orders them before the ticket).
         __shared__ int s_last;
         __threadfence();
         __syncthreads();
@@ -121,21 +126,24 @@ __global__ void __launch_bounds__(MK_THREADS, 2) k_merkle_chunk(const __grid_con
     if (a.root_out && tid == 0) merkle_publish_root(a, sm);
 }
 
-__global__ void k_merkle_paths(uint64_t *out, const uint64_t *tree, long long n, int depth,
-                               const uint64_t *indices, long long k) {
+// out[b][q][level] = word w of the sibling at `level` of leaf indices[q] in tree b (trees 2n nodes apart)
+__global__ void k_merkle_paths(uint64_t *out, const uint64_t *trees, long long n, int depth,
+                               const uint64_t *indices, long long k, long long batch) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = k * depth * 8;
+    const long long total = batch * k * depth * 8;
     if (t >= total) return;
     const int w = (int)(t & 7);
     const long long ql = t >> 3;
     const int level = (int)(ql % depth);
-    const long long q = ql / depth;
+    const long long qb = ql / depth, q = qb % k, b = qb / k;
     const long long node = ((n + (long long)indices[q]) >> level) ^ 1;
-    out[t] = tree[node * 8 + w];
+    out[t] = trees[(b * 2 * n + node) * 8 + w];
 }
-__global__ void k_gather(fe *out, const fe *values, const uint64_t *indices, long long k) {
+// out[b][q] = values[b * n + indices[q]]
+__global__ void k_gather(fe *out, const fe *values, long long n, const uint64_t *indices, long long k,
+                         long long batch) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < k) tile_st(out + t, tile_ld(values + indices[t]));
+    if (t < batch * k) tile_st(out + t, tile_ld(values + (t / k) * n + indices[t % k]));
 }
 
 // blake2b-only roof of the Merkle kernels: every thread hashes a chain of node messages (128 bytes = one
@@ -191,87 +199,131 @@ struct XinvTable : DeviceTables {
 using XinvPtr = std::shared_ptr<XinvTable>;
 
 // ---- Merkle / FRI ----
-// arrival counters of k_merkle_chunk's fused top, one per (device, stream): zero whenever no launch
-// of that stream is in flight (the last CTA resets it)
+// arrival counters of k_merkle_chunk's fused top, one per tree of a launch, per (device, stream): zero
+// whenever no launch of that stream is in flight (the last CTA of a tree resets its counter).  They grow
+// in 256-byte steps and never shrink.
+struct Tickets {
+    unsigned int *ptr = nullptr;
+    int count = 0;
+};
 static std::mutex g_tickets_mu;
-static std::map<std::pair<int, cudaStream_t>, unsigned int *> g_tickets;
-static unsigned int *get_ticket(cudaStream_t st) {
+static std::map<std::pair<int, cudaStream_t>, Tickets> g_tickets;
+static unsigned int *get_tickets(cudaStream_t st, int trees) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
     std::lock_guard<std::mutex> lock(g_tickets_mu);
-    auto &slot = g_tickets[std::make_pair(dev, st)];
-    if (!slot) {
-        if (cudaMalloc((void **)&slot, 256) != cudaSuccess || cudaMemset(slot, 0, 256) != cudaSuccess) {
-            slot = nullptr;
+    Tickets &slot = g_tickets[std::make_pair(dev, st)];
+    if (slot.count < trees) {
+        const int count = (trees + 63) / 64 * 64;
+        // earlier launches on this stream may still count on the old counters
+        if (slot.ptr && (cudaStreamSynchronize(st) != cudaSuccess || cudaFree(slot.ptr) != cudaSuccess)) {
             cudaGetLastError();
+            return nullptr;  // (the counters stay as they are)
+        }
+        slot = Tickets();
+        if (cudaMalloc((void **)&slot.ptr, 4 * (size_t)count) != cudaSuccess ||
+            cudaMemsetAsync(slot.ptr, 0, 4 * (size_t)count, st) != cudaSuccess) {
+            if (slot.ptr) cudaFree(slot.ptr);
+            slot = Tickets();
+            cudaGetLastError();
+        } else {
+            slot.count = count;
         }
     }
-    return slot;  // nullptr: fall back to one more launch
+    return slot.ptr;  // nullptr: fall back to one more launch
 }
-static int merkle_reduce(MerkleArgs a, cudaStream_t st, uint64_t *root_host = nullptr, unsigned long long seq = 0) {
+// the launches of `batch` trees, merkle_view's layout; root_host: publish the root of a single tree there
+static int merkle_reduce(MerkleArgs a, size_t batch, cudaStream_t st, uint64_t *root_host = nullptr,
+                         unsigned long long seq = 0) {
 #ifdef SA_TUNE
     const char *shape_spec = getenv("SA_MK_SHAPE");  // see merkle_shape_override
 #else
     const char *shape_spec = nullptr;
 #endif
-    return merkle_launches(a, get_ticket(st), shape_spec, [&](MerkleArgs &m, bool last) -> int {
-        m.root_out = last ? root_host : nullptr;
-        m.root_seq = seq;
-        k_merkle_chunk<<<(unsigned)(m.width / m.chunk), MK_THREADS, 0, st>>>(m);
-        SA_LAUNCH_CHECK();
-        return SA_OK;
-    });
+    if (root_host && batch != 1) return SA_ESIZE;
+    return merkle_batch_launches(
+        a, (long long)batch, [&](int trees) { return get_tickets(st, trees); }, shape_spec,
+        [&](MerkleArgs &m, int trees, bool last) -> int {
+            m.root_out = last ? root_host : nullptr;
+            m.root_seq = seq;
+            k_merkle_chunk<<<dim3((unsigned)(m.width / m.chunk), (unsigned)trees), MK_THREADS, 0, st>>>(m);
+            SA_LAUNCH_CHECK();
+            return SA_OK;
+        });
 }
 
 extern "C" {
 
-int sa_merkle_tree(void *tree, const void *values, size_t n, void *stream) {
+int sa_merkle_tree_batch(void *trees, const void *values, size_t n, size_t batch, void *stream) {
     if (!host_is_pow2(n)) return SA_ENOTPOW2;
-    cudaStream_t st = (cudaStream_t)stream;
-    SA_CUDA(cudaMemsetAsync(tree, 0, 64, st));
+    if (batch == 0) return SA_OK;
     MerkleArgs a;
     memset(&a, 0, sizeof(a));
-    a.tree = (uint64_t *)tree;
+    a.tree = (uint64_t *)trees;
+    a.tree_stride = 16 * (long long)n;
+    a.row_stride = (long long)n;
     a.width = (long long)n;
     a.mode = 1;
     a.values = (const fe *)values;
-    return merkle_reduce(a, st);
+    return merkle_reduce(a, batch, (cudaStream_t)stream);
+}
+
+int sa_merkle_tree(void *tree, const void *values, size_t n, void *stream) {
+    return sa_merkle_tree_batch(tree, values, n, 1, stream);
+}
+
+// checks the k leaf indices against n and, when the call has work (`work`, k > 0), uploads them to
+// stream-ordered device memory; *idx stays nullptr otherwise
+static int upload_indices(uint64_t **idx, const uint64_t *indices_host, size_t k, size_t n, bool work,
+                          cudaStream_t st) {
+    for (size_t i = 0; i < k; i++)
+        if (indices_host[i] >= n) return SA_EINDEX;
+    *idx = nullptr;
+    if (!work || k == 0) return SA_OK;
+    keep_pool_memory();
+    SA_CUDA(cudaMallocAsync((void **)idx, 8 * k, st));
+    SA_CUDA(cudaMemcpyAsync(*idx, indices_host, 8 * k, cudaMemcpyHostToDevice, st));
+    return SA_OK;
+}
+
+int sa_merkle_open_batch(void *paths_out, const void *trees, size_t n, size_t batch, const uint64_t *indices_host,
+                         size_t k, void *stream) {
+    if (!host_is_pow2(n)) return SA_ENOTPOW2;
+    const int depth = host_log2(n);
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t *idx = nullptr;
+    int rc = upload_indices(&idx, indices_host, k, n, batch != 0 && depth != 0, st);
+    if (rc != SA_OK || idx == nullptr) return rc;
+    const long long total = (long long)batch * (long long)k * depth * 8;
+    k_merkle_paths<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((uint64_t *)paths_out,
+                                                                    (const uint64_t *)trees, (long long)n,
+                                                                    depth, idx, (long long)k, (long long)batch);
+    SA_LAUNCH_CHECK();
+    cudaFreeAsync(idx, st);
+    return SA_OK;
 }
 
 int sa_merkle_open(void *paths_out, const void *tree, size_t n, const uint64_t *indices_host, size_t k,
                    void *stream) {
-    if (!host_is_pow2(n)) return SA_ENOTPOW2;
-    for (size_t i = 0; i < k; i++)
-        if (indices_host[i] >= n) return SA_EINDEX;
-    const int depth = host_log2(n);
-    if (k == 0 || depth == 0) return SA_OK;
+    return sa_merkle_open_batch(paths_out, tree, n, 1, indices_host, k, stream);
+}
+
+int sa_gather_batch(void *out, const void *values, size_t n, size_t batch, const uint64_t *indices_host, size_t k,
+                    void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     uint64_t *idx = nullptr;
-    keep_pool_memory();
-    SA_CUDA(cudaMallocAsync((void **)&idx, 8 * k, st));
-    SA_CUDA(cudaMemcpyAsync(idx, indices_host, 8 * k, cudaMemcpyHostToDevice, st));
-    const long long total = (long long)k * depth * 8;
-    k_merkle_paths<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((uint64_t *)paths_out,
-                                                                    (const uint64_t *)tree, (long long)n,
-                                                                    depth, idx, (long long)k);
+    int rc = upload_indices(&idx, indices_host, k, n, batch != 0, st);
+    if (rc != SA_OK || idx == nullptr) return rc;
+    const long long total = (long long)batch * (long long)k;
+    k_gather<<<(unsigned)((total + 127) / 128), 128, 0, st>>>((fe *)out, (const fe *)values, (long long)n, idx,
+                                                            (long long)k, (long long)batch);
     SA_LAUNCH_CHECK();
     cudaFreeAsync(idx, st);
     return SA_OK;
 }
 
 int sa_gather(void *out, const void *values, size_t n, const uint64_t *indices_host, size_t k, void *stream) {
-    for (size_t i = 0; i < k; i++)
-        if (indices_host[i] >= n) return SA_EINDEX;
-    if (k == 0) return SA_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    uint64_t *idx = nullptr;
-    keep_pool_memory();
-    SA_CUDA(cudaMallocAsync((void **)&idx, 8 * k, st));
-    SA_CUDA(cudaMemcpyAsync(idx, indices_host, 8 * k, cudaMemcpyHostToDevice, st));
-    k_gather<<<(unsigned)((k + 127) / 128), 128, 0, st>>>((fe *)out, (const fe *)values, idx, (long long)k);
-    SA_LAUNCH_CHECK();
-    cudaFreeAsync(idx, st);
-    return SA_OK;
+    return sa_gather_batch(out, values, n, 1, indices_host, k, stream);
 }
 
 // x_i^-1 tables: xinv[i] = omega^-i (Montgomery), i < n/2, cached per (device, omega, n) in the LRU above
@@ -323,7 +375,7 @@ int sa_fri_round(void *next, void *next_tree, const void *cw, size_t n, const ui
     a.next = (fe *)next;
     a.xinv = xinv->tab;
     fri_fold_scalars(&a.s_m, &a.inv2_m, fe_from_limbs(alpha), fe_mont_inv(fe_to_mont(fe_from_limbs(offset))));
-    return merkle_reduce(a, st);
+    return merkle_reduce(a, 1, st);
 }
 
 // spin until the kernel has published root number `seq` (see merkle_publish_root); the stream is
@@ -385,7 +437,7 @@ int sa_fri_commit(void *layers, void *trees, const void *codeword, size_t n, int
             a.width = (long long)len;
             a.mode = 1;
             a.values = cur;
-            if ((rc = merkle_reduce(a, st, root_dev, ++root_seq)) != SA_OK) return rc;
+            if ((rc = merkle_reduce(a, 1, st, root_dev, ++root_seq)) != SA_OK) return rc;
         }
         const double t_launched = now();
         if ((rc = wait_for_root(root_pinned, root_seq, st)) != SA_OK) return rc;
@@ -413,7 +465,7 @@ int sa_fri_commit(void *layers, void *trees, const void *codeword, size_t n, int
         a.next = layer_out;
         a.xinv = xinv->tab;
         fri_fold_scalars(&a.s_m, &a.inv2_m, fe_from_limbs(alpha), oinv_m);
-        if ((rc = merkle_reduce(a, st, root_dev, ++root_seq)) != SA_OK) return rc;
+        if ((rc = merkle_reduce(a, 1, st, root_dev, ++root_seq)) != SA_OK) return rc;
         cur = layer_out;
         layer_out += len / 2;
         tree = next_tree;

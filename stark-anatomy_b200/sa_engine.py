@@ -67,6 +67,9 @@ SYMBOLS = [
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
+    ("sa_merkle_tree_batch", _ci, [_vp, _vp, _sz, _sz, _vp]),
+    ("sa_merkle_open_batch", _ci, [_vp, _vp, _sz, _sz, _u64p, _sz, _vp]),
+    ("sa_gather_batch", _ci, [_vp, _vp, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_commit", _ci, [_vp, _vp, _vp, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
@@ -408,6 +411,63 @@ class CudaEngine:
             self._check(self.lib.sa_gather(out.data_ptr(), vec.data_ptr(), vec.shape[0], idx, k, self._stream()))
             self._count("h2d", 8 * k)
             self._count("d2h", 16 * k)
+        return out.cpu().numpy()
+
+    def merkle_trees(self, vecs):
+        """sa_merkle_tree_batch: the trees of B codewords of one length n, (B, n, 2) -> (B, 2n, 64) uint8, in one
+        launch ladder; asynchronous"""
+        if vecs.dim() != 3 or vecs.shape[-1] != 2:  # the library cannot see the tensor's shape
+            raise SaError(SA_ERRORS[-6])
+        vecs = vecs.contiguous()
+        batch, n = vecs.shape[0], vecs.shape[1]
+        trees = self.torch.empty((batch, 2 * n, 64), dtype=self.torch.uint8, device=self.device)
+        self._check(self.lib.sa_merkle_tree_batch(trees.data_ptr(), vecs.data_ptr(), n, batch, self._stream()))
+        return trees
+
+    def tree_roots(self, trees):
+        """the roots of a (B, 2n, 64) batch of trees as B 64-byte strings, from one device-to-host copy"""
+        if trees.dim() != 3 or trees.shape[1] < 2 or trees.shape[1] % 2 or trees.shape[2] != 64:
+            raise SaError(SA_ERRORS[-6])
+        self._count("d2h", 64 * trees.shape[0])
+        raw = trees[:, 1].cpu().numpy().tobytes()
+        return [raw[64 * b:64 * (b + 1)] for b in range(trees.shape[0])]
+
+    def merkle_open_batch(self, trees, indices):
+        """sa_merkle_open_batch: for each tree of a (B, 2n, 64) batch, the authentication paths of the same leaf
+        indices (B lists of k lists of 64-byte digests, bottom-up), with one upload and one download"""
+        if trees.dim() != 3 or trees.shape[1] < 2 or trees.shape[1] % 2 or trees.shape[2] != 64:
+            raise SaError(SA_ERRORS[-6])
+        trees = trees.contiguous()
+        batch, n, k = trees.shape[0], trees.shape[1] // 2, len(indices)
+        depth = n.bit_length() - 1
+        for i in indices:
+            if not 0 <= i < n:
+                raise SaError(SA_ERRORS[-5])
+        out = self.torch.empty((batch, k, depth, 64), dtype=self.torch.uint8, device=self.device)
+        idx = (ctypes.c_uint64 * k)(*indices)
+        self._check(self.lib.sa_merkle_open_batch(out.data_ptr(), trees.data_ptr(), n, batch, idx, k, self._stream()))
+        if out.numel() == 0:  # no tree, no index or no sibling: nothing was launched
+            return [[[] for _ in indices] for _ in range(batch)]
+        self._count("h2d", 8 * k)
+        self._count("d2h", out.numel())
+        raw = out.cpu().numpy().tobytes()
+        digests = [raw[i:i + 64] for i in range(0, len(raw), 64)]
+        paths = [digests[i:i + depth] for i in range(0, len(digests), depth)]
+        return [paths[b * k:(b + 1) * k] for b in range(batch)]
+
+    def gather_batch(self, vecs, indices):
+        """sa_gather_batch: the values at the same indices in each row of a (B, n, 2) batch -> numpy (B, k, 2) on
+        the host (the int64 limbs `gather` returns), with one upload and one download"""
+        if vecs.dim() != 3 or vecs.shape[-1] != 2:
+            raise SaError(SA_ERRORS[-6])
+        vecs = vecs.contiguous()
+        batch, n, k = vecs.shape[0], vecs.shape[1], len(indices)
+        out = self.torch.empty((batch, k, 2), dtype=self.torch.int64, device=self.device)
+        idx = (ctypes.c_uint64 * k)(*indices)
+        self._check(self.lib.sa_gather_batch(out.data_ptr(), vecs.data_ptr(), n, batch, idx, k, self._stream()))
+        if out.numel():
+            self._count("h2d", 8 * k)
+            self._count("d2h", out.numel() * 8)
         return out.cpu().numpy()
 
     # ------------------------------------------------------------------ fri
