@@ -215,6 +215,25 @@ int sa_coset_div_apply_batch(void *out, const void *plan, const void *lhs, size_
  * coeffs.                                                                                        */
 int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log_n, const uint64_t root[2],
                             const uint64_t offset[2], size_t batch, void *stream);
+/* code/fast_stark.py:125-148: the weighted, degree-shifted combination of many device polynomials and its
+ * fast_coset_evaluate, in one call.  With n = 2^log_n, c[i] = sum_t w_t * srcs[t][i - shifts[t]] over the terms t
+ * with shifts[t] <= i < shifts[t] + lens[t], and out[0..n) = ntt(c[i] * offset^i, zero padded to n): the
+ * reference's combined_codeword for the same terms (x^s * q is q at shift s).  Term t is a DEVICE row of lens[t]
+ * elements (rows may be slices of different buffers, and several terms may share one row), a shift and the weight
+ * weights[2t], weights[2t+1] (the limbs of a canonical residue).  srcs, lens, shifts and weights are HOST arrays,
+ * read before the call returns: the terms travel as kernel parameters, so the call uploads nothing.  A term with
+ * lens[t] == 0 adds nothing; nterms == 0 writes n zeros (the empty combination).
+ * Before any launch: SA_ESIZE for log_n outside 1..30 or any shifts[t] + lens[t] > n, and the root's
+ * SA_EROOTORDER / SA_ENOTPRIM as for sa_coset_evaluate_batch.  Every offset is accepted, 0 included.
+ * out must not overlap any source.  Launches: one offset^i table of ncomb = max_t(shifts[t] + lens[t]) elements
+ * (per-stream workspace), one per group of 64 terms, one forward sa_ntt in place on out: 1 + ceil(nterms / 64)
+ * plus the transform's (none but the group launches when ncomb == 0).  Asynchronous: no host synchronisation,
+ * and no allocation once the stream's workspaces have grown for this ncomb and log_n, so the call can be
+ * captured in a CUDA graph after one call on the capturing stream (the same conditions as
+ * sa_coset_div_apply_batch); a replay uses the terms (rows, lengths, shifts, weights) it was captured with.   */
+int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                              const void *const *srcs, const size_t *lens, const size_t *shifts,
+                              const uint64_t *weights, size_t nterms, void *stream);
 /* The most rows one chunk of sa_coset_div_apply_batch / sa_coset_evaluate_batch takes:
  * max(1, floor(2^30 / (32 n))) (32 at 2^20, 512 at 2^16), so a chunk's workspace stays at or below
  * 1 GiB; 0 when log_n is outside 1..30.  Host-only: no CUDA call.                                */

@@ -1,6 +1,7 @@
 // coset.cuh -- division by one polynomial on a coset, many numerators at a time (fast_coset_divide,
-// code/ntt.py:137-176), and batched coset evaluation (fast_coset_evaluate, ntt.py:132-135): the per-element bodies
-// of their kernels and the host schedules of the plan build, the apply and the evaluation.  The library (poly.cu)
+// code/ntt.py:137-176), batched coset evaluation (fast_coset_evaluate, ntt.py:132-135) and the coset evaluation of a
+// weighted, degree-shifted sum of many polynomials (fast_stark.py:125-148): the per-element bodies of their kernels
+// and the host schedules of the plan build, the apply, the evaluation and the combination.  The library (poly.cu)
 // runs the schedules with kernel launches, the CPU emulation (tests/emu) with loops over the element functions.
 //
 // The schedules take the backend of poly_tree.cuh (one method per kernel, named after it without the k_ prefix:
@@ -36,6 +37,36 @@ SA_HD void coset_quot_elem(fe *ws, const fe *inv_m, int log_n, long long idx) {
 SA_HD void coset_store_elem(fe *out, const fe *ws, const fe *ipw_m, long long qlen, int log_n, long long idx) {
     const long long b = idx >> log_n, j = idx & ((1ll << log_n) - 1);
     if (j < qlen) tile_st(out + b * qlen + j, fe_montmul(tile_ld(ws + idx), tile_ld(ipw_m + j)));
+}
+
+// A group of a combination's terms, taken by one launch as a kernel parameter (__grid_constant__: 2.5 KB, inside the
+// classic 4 KB parameter limit).  Term t is the row src[0..len) shifted up by `shift`, weighted by w_m (Montgomery
+// form, so each covered index costs one fe_montmul and one fe_add).
+constexpr int COMBINE_TERMS = 64;
+struct CombineTerm {
+    const fe *src;
+    long long len, shift;
+    fe w_m;
+};
+struct CombineGroup {
+    CombineTerm t[COMBINE_TERMS];
+    int count;
+};
+// out[i] (+)= offset^i * sum_t w_t * src_t[i - shift_t] over the group's terms whose window covers i, for i < ncomb;
+// the first group (first != 0) writes every i < n, zero from ncomb on, each later one adds its own scaled sum
+// (scaling by offset^i is linear)  (idx < n)
+SA_HD void coset_combine_elem(fe *out, const CombineGroup &g, const fe *pw_m, long long ncomb, int first, long long i) {
+    if (i >= ncomb) {
+        if (first) tile_st(out + i, fe_zero());
+        return;
+    }
+    fe s = fe_zero();
+    for (int t = 0; t < g.count; t++) {
+        const long long j = i - g.t[t].shift;
+        if (j >= 0 && j < g.t[t].len) s = fe_add(s, fe_montmul(tile_ld(g.t[t].src + j), g.t[t].w_m));
+    }
+    s = fe_montmul(s, tile_ld(pw_m + i));
+    tile_st(out + i, first ? s : fe_add(tile_ld(out + i), s));
 }
 
 // ---- host schedule ----
@@ -135,6 +166,47 @@ int coset_evaluate(B &b, fe *out, const fe *coeffs, size_t ncoef, int log_n, con
         SA_TRY(b.ntt(out + b0 * n, out + b0 * n, log_n, root, 0, nb));
     }
     return SA_OK;
+}
+
+// ---- coset combinations (the combination of fast_stark.py:125-148 and its fast_coset_evaluate) ----
+// ncomb = max_t(shifts[t] + lens[t]): the combination's length, and the offset^i its schedule tables
+inline size_t coset_combine_len(const size_t *lens, const size_t *shifts, size_t nterms) {
+    size_t m = 0;
+    for (size_t t = 0; t < nterms; t++) m = std::max(m, shifts[t] + lens[t]);
+    return m;
+}
+// the checks of a combination, before its workspace is taken and before its first launch: the size, every term's
+// window inside [0, n) and the root (sa_ntt's SA_EROOTORDER / SA_ENOTPRIM).  Every offset is accepted, 0 included.
+inline int coset_combine_check(int log_n, const size_t *lens, const size_t *shifts, size_t nterms,
+                               const uint64_t root[2]) {
+    if (log_n < 1 || log_n > COSET_MAX_LOG) return SA_ESIZE;
+    const size_t n = (size_t)1 << log_n;
+    for (size_t t = 0; t < nterms; t++)
+        if (shifts[t] > n || lens[t] > n - shifts[t]) return SA_ESIZE;
+    return ntt_check_root(fe_to_mont(fe_from_limbs(root)), log_n);
+}
+
+// out = ntt(c[i] * offset^i, zero padded to n), c[i] = sum_t w_t * srcs[t][i - shifts[t]] over the terms with
+// shifts[t] <= i < shifts[t] + lens[t] (fast_coset_evaluate of the combination at order n): offset^i for i < ncomb
+// into pw (ncomb elements), then the terms in groups of COMBINE_TERMS, one launch each (the first writes all of out,
+// the others add), then one transform in place -- 1 + ceil(nterms / 64) launches plus the transform's.  With
+// ncomb == 0 (no term, or only empty ones at shift 0) out is n zeros from the group launches alone: no table, no
+// transform.  out must not overlap any source.
+template <class B>
+int coset_combine_evaluate(B &b, fe *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                           const fe *const *srcs, const size_t *lens, const size_t *shifts, const uint64_t *weights,
+                           size_t nterms, fe *pw) {
+    const long long ncomb = (long long)coset_combine_len(lens, shifts, nterms);
+    if (ncomb) SA_TRY(b.pow_table(pw, fe_to_mont(fe_from_limbs(offset)), ncomb));
+    for (size_t t0 = 0; t0 == 0 || t0 < nterms; t0 += COMBINE_TERMS) {
+        CombineGroup g;
+        g.count = (int)std::min((size_t)COMBINE_TERMS, nterms - t0);
+        for (int k = 0; k < g.count; k++)
+            g.t[k] = CombineTerm{srcs[t0 + k], (long long)lens[t0 + k], (long long)shifts[t0 + k],
+                                 fe_to_mont(fe_from_limbs(weights + 2 * (t0 + k)))};
+        SA_TRY(b.coset_combine(out, g, pw, ncomb, log_n, t0 == 0));
+    }
+    return ncomb ? b.ntt(out, out, log_n, root, 0, 1) : SA_OK;
 }
 
 }  // namespace sa

@@ -1,7 +1,7 @@
 // poly.cu -- polynomial kernels: element-wise products, batch inversion, Horner evaluation, the
 // direct zerofier and Lagrange kernels, the kernels of the subproduct tree (poly_tree.cuh) behind
-// sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans and batched coset
-// evaluation (coset.cuh), with the backend that launches them for the headers' schedules.
+// sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans, batched coset
+// evaluation and coset combinations (coset.cuh), with the backend that launches them for the headers' schedules.
 //
 // Reference behaviour reproduced (bit-exact): code/ntt.py:61-176, code/algebra.py:53-57,75-94.
 #include <algorithm>
@@ -208,6 +208,11 @@ __global__ void k_coset_quot(fe *ws, const fe *inv_m, int log_n, long long batch
 __global__ void k_coset_store(fe *out, const fe *ws, const fe *ipw_m, long long qlen, int log_n, long long batch) {
     grid_stride(batch << log_n, [&](long long idx) { coset_store_elem(out, ws, ipw_m, qlen, log_n, idx); });
 }
+// one group of a combination's terms over all n outputs; the group is a kernel parameter, so the call uploads nothing
+__global__ void k_coset_combine(fe *out, const __grid_constant__ CombineGroup g, const fe *pw_m, long long ncomb,
+                                int log_n, int first) {
+    grid_stride(1ll << log_n, [&](long long i) { coset_combine_elem(out, g, pw_m, ncomb, first, i); });
+}
 
 extern "C" {
 
@@ -285,6 +290,9 @@ struct DeviceTree {
     int coset_quot(fe *ws, const fe *inv, int lg, ll nb) { return go(k_coset_quot, tree_grid(nb << lg), ws, inv, lg, nb); }
     int coset_store(fe *o, const fe *ws, const fe *ipw, ll q, int lg, ll nb) {
         return go(k_coset_store, tree_grid(nb << lg), o, ws, ipw, q, lg, nb);
+    }
+    int coset_combine(fe *o, const CombineGroup &g, const fe *pw, ll nc, int lg, int first) {
+        return go(k_coset_combine, tree_grid(1ll << lg), o, g, pw, nc, lg, first);
     }
     int ntt(fe *o, const fe *i, int lg, const uint64_t *r, int inv, size_t nb) { return sa_ntt(o, i, lg, r, inv, nb, st); }
     int copy(fe *dst, const fe *src, size_t n) {
@@ -492,6 +500,20 @@ int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log
     SA_TRY(get_workspace((void **)&pw, sizeof(fe) * ncoef, st, WS_COSET));
     DeviceTree b{st};
     return coset_evaluate(b, (fe *)out, (const fe *)coeffs, ncoef, log_n, root, offset, batch, pw);
+}
+
+// scratch: offset^i for i < ncomb (WS_COSET); the terms travel as kernel parameters and out is transformed in place
+int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                              const void *const *srcs, const size_t *lens, const size_t *shifts,
+                              const uint64_t *weights, size_t nterms, void *stream) {
+    SA_TRY(coset_combine_check(log_n, lens, shifts, nterms, root));
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *pw = nullptr;
+    const size_t ncomb = coset_combine_len(lens, shifts, nterms);
+    if (ncomb) SA_TRY(get_workspace((void **)&pw, sizeof(fe) * ncomb, st, WS_COSET));
+    DeviceTree b{st};
+    return coset_combine_evaluate(b, (fe *)out, log_n, root, offset, (const fe *const *)srcs, lens, shifts, weights,
+                                  nterms, pw);
 }
 
 }  // extern "C"

@@ -64,6 +64,8 @@ SYMBOLS = [
     ("sa_coset_div_apply_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _ci, _u64p, _sz, _vp]),
     ("sa_coset_evaluate_batch", _ci, [_vp, _vp, _sz, _ci, _u64p, _u64p, _sz, _vp]),
     ("sa_coset_batch_max", _sz, [_ci]),
+    ("sa_coset_combine_evaluate", _ci, [_vp, _ci, _u64p, _u64p, ctypes.POINTER(ctypes.c_void_p),
+                                        ctypes.POINTER(_sz), ctypes.POINTER(_sz), _u64p, _sz, _vp]),
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
@@ -355,6 +357,35 @@ class CudaEngine:
         if batch:
             self._check(self.lib.sa_coset_evaluate_batch(out.data_ptr(), coeffs.data_ptr(), coeffs.shape[-2], log_n,
                                                          _limbs(root), _limbs(offset), batch, self._stream()))
+        return out
+
+    def coset_combine_evaluate(self, terms, log_n, root, offset):
+        """sa_coset_combine_evaluate: fast_coset_evaluate at order 2^log_n of sum_t weight_t * X^shift_t * vec_t over
+        terms (vec, shift, weight), each vec a contiguous int64 (len, 2) tensor on this device -> (n, 2) in one call
+        (the combination of fast_stark.py:125-148); asynchronous, nothing is uploaded"""
+        torch = self.torch
+        if self.lib.sa_coset_batch_max(log_n) == 0:
+            raise SaError(SA_ERRORS[-6])
+        n = 1 << log_n
+        ptrs, lens, shifts, weights = [], [], [], []
+        for vec, shift, weight in terms:  # the library cannot see the tensors' shape, device or layout
+            if (not isinstance(vec, torch.Tensor) or vec.dtype != torch.int64 or vec.dim() != 2 or vec.shape[1] != 2
+                    or vec.device != self.device or not vec.is_contiguous()):
+                raise SaError(SA_ERRORS[-6])
+            shift = int(shift)
+            if shift < 0 or shift + vec.shape[0] > n:
+                raise SaError(SA_ERRORS[-6])
+            weight = int(weight) % P
+            ptrs.append(vec.data_ptr())
+            lens.append(vec.shape[0])
+            shifts.append(shift)
+            weights += [weight & 0xFFFFFFFFFFFFFFFF, weight >> 64]
+        t = len(ptrs)
+        out = self.empty(n)
+        self._check(self.lib.sa_coset_combine_evaluate(
+            out.data_ptr(), log_n, _limbs(root), _limbs(offset), (ctypes.c_void_p * t)(*ptrs),
+            (ctypes.c_size_t * t)(*lens), (ctypes.c_size_t * t)(*shifts), (ctypes.c_uint64 * (2 * t))(*weights), t,
+            self._stream()))
         return out
 
     # --------------------------------------------------------------- merkle
