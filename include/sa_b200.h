@@ -239,6 +239,43 @@ int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], cons
  * 1 GiB; 0 when log_n is outside 1..30.  Host-only: no CUDA call.                                */
 size_t sa_coset_batch_max(int log_n);
 
+/* ---- code/fast_stark.py:108-113: the transition quotients of an AIR, without symbolic polynomials -------------
+ * The constraints are polynomials in nvars = 1 + 2*nregs variables in FastStark's order: x, the trace rows T_s(x)
+ * (variables 1..nregs) and the next rows T_s(step*x) (variables nregs+1..2*nregs).  Constraint c is the terms
+ * term_start[c] .. term_start[c+1]; term t has the coefficient coeffs[2t], coeffs[2t+1] (the limbs of a canonical
+ * residue) and the exponents exps[t*nvars .. t*nvars + nvars).  A constraint without terms is the zero polynomial.
+ * With n = 2^log_n, x_i = offset * root^i and N_c(x) = C_c(x, T(x), T(step*x)), row c of an apply is
+ *     out[c][j] = U_c[j] * offset^-j  (j < qlen),   U_c = intt(N_c(x_i) / Z(x_i)),
+ * the numerator evaluated point by point on the coset and divided there.  Where every term's degree bound
+ * e_0 + (e_1 + ... + e_2nregs) * (max_ncoef - 1) is below n (the build refuses anything else), N_c is the
+ * polynomial MPolynomial.evaluate_symbolic gives, and out[c][0 .. deg N_c - deg Z] is fast_coset_divide's quotient
+ * at order n, bit for bit, clean division or not.
+ * A plan holds the zerofier's coset division plan, (offset*step)^j, the points x_i and the constraints compiled into
+ * a program.  It is a device buffer the caller owns, of sa_air_plan_bytes(log_n, max_ncoef, nregs, nterms) bytes
+ * with nterms = term_start[ncons]: 80*n + 16*sec16(1 + nterms*(2 + ceil(nregs/2))) from n = 16 on, sec16 rounding up
+ * to a multiple of 16 (DESIGN section 2).  0 when log_n is outside 1..30, nregs == 0, max_ncoef is outside 1..n or
+ * nterms >= 2^32.  Host-only: no CUDA call.                                                                     */
+size_t sa_air_plan_bytes(int log_n, size_t max_ncoef, size_t nregs, size_t nterms);
+/* Builds the plan.  coeffs, exps and term_start are HOST arrays, compiled into the plan; zerofier[0..zlen) is a
+ * device row.  Before any launch: SA_ESIZE for log_n outside 1..30, nregs == 0, ncons == 0, max_ncoef or zlen outside
+ * 1..n, a decreasing term_start, or a term whose degree bound (above) is >= n; the root's SA_EROOTORDER /
+ * SA_ENOTPRIM.  SA_EDIVZERO when Z vanishes somewhere on the coset.  Every offset and step is accepted, 0 included.
+ * Synchronises (it reads the zero flag).                                                                       */
+int sa_air_plan(void *plan, const uint64_t *coeffs, const uint32_t *exps, const size_t *term_start, size_t ncons,
+                size_t nregs, size_t max_ncoef, const void *zerofier, size_t zlen, int log_n, const uint64_t root[2],
+                const uint64_t offset[2], const uint64_t step[2], void *stream);
+/* out[c*qlen .. c*qlen+qlen) = row c (above) for c < ncons, from trace[nregs][ncoef], the trace polynomials'
+ * coefficient rows (sa_interp_apply_batch's layout).  log_n, root, nregs and ncons must be the plan's and
+ * ncoef <= the plan's max_ncoef.  SA_ESIZE before any launch for nregs or ncons == 0 or ncoef, qlen outside 1..n.
+ * Rows are contiguous, so they feed sa_coset_combine_evaluate as they are.  Launches: two coset loads, one batched
+ * forward sa_ntt of the 2*nregs rows, then per chunk of sa_coset_batch_max(log_n) constraints the evaluation kernel,
+ * one batched inverse sa_ntt and the store -- the same count whatever nregs and the chunk's size.  Per-stream
+ * workspace: 16*n*(2*nregs + chunk) bytes besides the transform's.  Asynchronous: no host synchronisation, and no
+ * allocation once the stream's workspaces have grown, so the call can be captured in a CUDA graph (the same
+ * conditions as sa_coset_div_apply_batch).  Reads the plan only: one plan may be applied on several streams at once. */
+int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
+                     size_t ncons, int log_n, const uint64_t root[2], void *stream);
+
 /* ---- code/merkle.py:6-14 Merkle.commit -------------------------------------------------
  * Builds the whole blake2b-512 tree over n = 2^k leaves, leaf = H(decimal ASCII of the
  * value), node = H(left || right).  `tree` receives 2n nodes of 64 bytes in heap order:

@@ -1,0 +1,235 @@
+// air.cuh -- transition quotients of an AIR on a coset (fast_stark.py:108-113 without evaluate_symbolic): the
+// per-point body of k_air_eval, the plan layout, the checks, the host-side compilation of the constraints and the
+// host schedules of the plan build and the apply.  The library (poly.cu) runs the schedules with kernel launches, the
+// CPU emulation (tests/emu/emu_air.cpp) with loops over the element functions.
+//
+// The constraints are polynomials in nvars = 1 + 2 nregs variables, FastStark's point: x, the trace rows T_s(x) and
+// the next rows T_s(step * x).  With n = 2^log_n, x_i = offset * root^i and N_c(x) = C_c(x, T(x), T(step * x)), row c
+// of an apply is
+//     out[c][j] = U_c[j] * offset^-j  (j < qlen),   U_c = intt(N_c(x_i) / Z(x_i)),
+// the coset division of coset.cuh with the numerator's values computed point by point instead of transformed from
+// its coefficients.  Where every term's degree bound e_0 + (e_1 + ... + e_2nregs) (max_ncoef - 1) is below n (the
+// build checks it) N_c has degree < n, so its values determine it and the rows are fast_coset_divide's at order n,
+// bit for bit, clean division or not.
+//
+// The schedules take the backend of coset.cuh plus b.pow_table_lead(out, base_m, lead_m, count) (k_pow_table with a
+// lead), b.upload(dst, host_src, count) and b.air_eval (k_air_eval).
+#pragma once
+#include <algorithm>
+#include <cstdint>
+#include <numeric>
+#include <vector>
+
+#include "coset.cuh"
+
+namespace sa {
+
+// ---- the compiled program ----
+// Element 0 holds the record count (limbs 0, 1).  Record t is AIR_REC(nregs) elements:
+//   [0] header: v[0] = constraint, v[1] = AIR_FIRST | AIR_LAST flags, v[2] = x-exponent step, v[3] = 0
+//   [1] the coefficient (canonical)
+//   [2 ..] the group's trace exponents e_1 .. e_2nregs, four per element
+// Records run in constraint order; within a constraint the terms sharing one trace-exponent vector form a group, in
+// ascending x exponent.  The first record of a group steps from x^0, every other from the previous record's x power:
+// dense x-polynomials cost one product per term, a sparse high power O(log) products.
+constexpr uint32_t AIR_FIRST = 1, AIR_LAST = 2;
+inline size_t air_rec(size_t nregs) { return 2 + (nregs + 1) / 2; }
+
+// b^e, b and the result in Montgomery form, left to right from b itself: e == 1 costs no product, e == 0 gives 1
+SA_HD fe air_pow(const fe &b_m, uint32_t e) {
+    if (e == 0) return fe_mont_one();
+    int top = 31;
+    while (!((e >> top) & 1u)) top--;
+    fe acc = b_m;
+    for (int bit = top - 1; bit >= 0; bit--) {
+        acc = fe_montmul(acc, acc);
+        if ((e >> bit) & 1u) acc = fe_montmul(acc, b_m);
+    }
+    return acc;
+}
+
+// ---- element function: the body of k_air_eval for one point ----
+// V[c - c0][i] = N_c(x_i) / Z(x_i) for the constraints c0 <= c < c0 + nb, walking the program once: records of other
+// constraints are skipped, a constraint without records gets zeros.  x_m and iz_m are the plan's x_i and 1/Z_i, ext
+// the 2 nregs rows T_s(x_i), T_s(step * x_i) (canonical); coefficients are canonical, so a coefficient times a
+// Montgomery-form power is canonical again  (i < n)
+SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long c0,
+                         long long nb, int nregs, int log_n, long long i) {
+    const long long n = 1ll << log_n;
+    const fe x = tile_ld(x_m + i), iz = tile_ld(iz_m + i), h0 = tile_ldg(prog);
+    const long long nrec = (long long)h0.v[0] | (long long)h0.v[1] << 32, stride = 2 + (nregs + 1) / 2;
+    long long cur = c0;
+    fe acc = fe_zero(), s = fe_zero(), xp = fe_mont_one();
+    for (long long t = 0; t < nrec; t++) {
+        const fe *rec = prog + 1 + t * stride;
+        const fe h = tile_ldg(rec);
+        const long long c = h.v[0];
+        if (c < c0) continue;
+        if (c >= c0 + nb) break;
+        for (; cur < c; cur++, acc = fe_zero()) tile_st(V + (cur - c0) * n + i, fe_montmul(acc, iz));
+        if (h.v[1] & AIR_FIRST) {
+            xp = air_pow(x, h.v[2]);
+            s = fe_zero();
+        } else {
+            xp = fe_montmul(xp, air_pow(x, h.v[2]));
+        }
+        s = fe_add(s, fe_montmul(tile_ldg(rec + 1), xp));
+        if (h.v[1] & AIR_LAST) {
+            for (int w = 0; w < (nregs + 1) / 2; w++) {
+                const fe e4 = tile_ldg(rec + 2 + w);
+                for (int k = 0; k < 4; k++) {
+                    const int v = 4 * w + k;
+                    if (v < 2 * nregs && e4.v[k])
+                        s = fe_montmul(s, air_pow(fe_to_mont(tile_ld(ext + v * n + i)), e4.v[k]));
+                }
+            }
+            acc = fe_add(acc, s);
+        }
+    }
+    for (; cur < c0 + nb; cur++, acc = fe_zero()) tile_st(V + (cur - c0) * n + i, fe_montmul(acc, iz));
+}
+
+// ---- plan layout ----
+// A plan is a device buffer of air_plan_layout(...).elems elements; every section starts on a 256-byte (16-element)
+// boundary, S = sec16(n):
+//   offset^i | 1/Z_i | offset^-i   (the coset division plan of the zerofier, 3 S)
+//   (offset * step)^j, j < n       (S; the next rows' load)
+//   x_i = offset * root^i          (S)
+//   the program                    (sec16(1 + nterms * air_rec(nregs)))
+// all field sections in Montgomery form.  Every section but the program sits where log_n alone puts it, so an apply
+// finds them from (log_n, nregs) -- the arguments it has -- and the kernel reads the program's length from the plan.
+// 80 n + 16 sec16(1 + nterms (2 + ceil(nregs / 2))) bytes from n = 16 on.
+struct AirPlan {
+    int log_n = 0;
+    long long n = 0;
+    CosetPlan div;
+    size_t spw = 0, x = 0, prog = 0;  // element offsets of the sections after the division plan
+    size_t elems = 0;                 // 0: no plan for these sizes
+};
+constexpr size_t AIR_MAX_TERMS = (size_t)1 << 32;
+inline AirPlan air_plan_layout(int log_n, size_t max_ncoef, size_t nregs, size_t nterms) {
+    AirPlan L;
+    const CosetPlan d = coset_div_plan_layout(log_n);
+    if (d.elems == 0 || nregs == 0 || nregs > AIR_MAX_TERMS || max_ncoef < 1 || max_ncoef > (size_t)d.n ||
+        nterms >= AIR_MAX_TERMS)
+        return L;
+    L.log_n = log_n;
+    L.n = d.n;
+    L.div = d;
+    L.spw = d.elems;
+    L.x = L.spw + sec16((size_t)L.n);
+    L.prog = L.x + sec16((size_t)L.n);
+    L.elems = L.prog + sec16(1 + nterms * air_rec(nregs));
+    return L;
+}
+
+// An apply's workspace: the 2 nregs transformed rows and n elements per constraint row of a chunk (its chunks are
+// coset_batch_max(log_n) constraints); the transforms take the NTT's own besides.
+inline size_t air_chunk(size_t ncons, int log_n) { return std::min(ncons, coset_batch_max(log_n)); }
+inline size_t air_ws_elems(size_t nregs, size_t ncons, int log_n) {
+    return ((size_t)1 << log_n) * (2 * nregs + air_chunk(ncons, log_n));
+}
+
+// ---- checks, before any workspace is taken and before any launch ----
+// a build's: the sizes (log_n 1..30, nregs and ncons >= 1, max_ncoef and zlen 1..n), term_start non-decreasing, every
+// term's degree bound below n (pointwise evaluation is exact there) and the root (SA_EROOTORDER / SA_ENOTPRIM)
+inline int air_plan_check(int log_n, const uint32_t *exps, const size_t *term_start, size_t ncons, size_t nregs,
+                          size_t max_ncoef, size_t zlen, const uint64_t root[2]) {
+    if (log_n < 1 || log_n > COSET_MAX_LOG || nregs == 0 || ncons == 0) return SA_ESIZE;
+    const uint64_t n = (uint64_t)1 << log_n;
+    if (max_ncoef < 1 || max_ncoef > n || zlen < 1 || zlen > n) return SA_ESIZE;
+    for (size_t c = 0; c < ncons; c++)
+        if (term_start[c + 1] < term_start[c]) return SA_ESIZE;
+    if (air_plan_layout(log_n, max_ncoef, nregs, term_start[ncons]).elems == 0) return SA_ESIZE;
+    const size_t nvars = 1 + 2 * nregs;
+    for (size_t t = term_start[0]; t < term_start[ncons]; t++) {
+        const uint32_t *e = exps + t * nvars;
+        if (e[0] >= n) return SA_ESIZE;
+        uint64_t tdeg = 0;
+        for (size_t v = 1; v < nvars; v++) tdeg += e[v];
+        // e_0 + tdeg (max_ncoef - 1) < n, without overflow
+        if (max_ncoef > 1 && tdeg > (n - 1 - e[0]) / (max_ncoef - 1)) return SA_ESIZE;
+    }
+    return ntt_check_root(fe_to_mont(fe_from_limbs(root)), log_n);
+}
+// an apply's: the sizes (ncoef and qlen 1..n) and the root
+inline int air_apply_check(int log_n, size_t nregs, size_t ncoef, size_t qlen, size_t ncons, const uint64_t root[2]) {
+    if (nregs == 0 || ncons == 0) return SA_ESIZE;
+    return coset_check(log_n, ncoef, qlen, root);
+}
+
+// ---- compilation (host) ----
+// the program of the terms term_start[0] .. term_start[ncons): the terms of each constraint sorted by (trace
+// exponents, x exponent), grouped by trace exponents, x steps taken within a group
+inline std::vector<fe> air_compile(const uint64_t *coeffs, const uint32_t *exps, const size_t *term_start, size_t ncons,
+                                   size_t nregs) {
+    const size_t nvars = 1 + 2 * nregs, rec = air_rec(nregs), nterms = term_start[ncons] - term_start[0];
+    std::vector<fe> prog(1 + nterms * rec, fe_zero());
+    prog[0] = fe_make((uint32_t)nterms, (uint32_t)((uint64_t)nterms >> 32), 0, 0);
+    auto same_trace = [&](size_t a, size_t b) {
+        return std::equal(exps + a * nvars + 1, exps + (a + 1) * nvars, exps + b * nvars + 1);
+    };
+    size_t r = 0;
+    for (size_t c = 0; c < ncons; c++) {
+        std::vector<size_t> ts(term_start[c + 1] - term_start[c]);
+        std::iota(ts.begin(), ts.end(), term_start[c]);
+        std::stable_sort(ts.begin(), ts.end(), [&](size_t a, size_t b) {
+            return std::lexicographical_compare(exps + a * nvars + 1, exps + (a + 1) * nvars, exps + b * nvars + 1,
+                                                exps + (b + 1) * nvars) ||
+                   (same_trace(a, b) && exps[a * nvars] < exps[b * nvars]);
+        });
+        for (size_t k = 0; k < ts.size(); k++, r++) {
+            const size_t t = ts[k];
+            const bool first = k == 0 || !same_trace(ts[k - 1], t);
+            const bool last = k + 1 == ts.size() || !same_trace(t, ts[k + 1]);
+            const uint32_t dx = first ? exps[t * nvars] : exps[t * nvars] - exps[ts[k - 1] * nvars];
+            fe *p = prog.data() + 1 + r * rec;
+            p[0] = fe_make((uint32_t)c, (first ? AIR_FIRST : 0) | (last ? AIR_LAST : 0), dx, 0);
+            p[1] = fe_from_limbs(coeffs + 2 * t);
+            for (size_t v = 0; v < 2 * nregs; v++) p[2 + v / 4].v[v % 4] = exps[t * nvars + 1 + v];
+        }
+    }
+    return prog;
+}
+
+// ---- host schedules ----
+// The plan: the zerofier's coset division plan (coset_div_plan_build, ws = n elements), (offset * step)^j, x_i and
+// the program compiled on the host and uploaded.  The caller reads *flag after the build (SA_EDIVZERO when Z vanishes
+// on the coset) and keeps `prog` alive until the upload has completed.
+template <class B>
+int air_plan_build(B &b, fe *plan, const std::vector<fe> &prog, const fe *zerofier, size_t zlen, int log_n,
+                   const uint64_t root[2], const uint64_t offset[2], const uint64_t step[2], fe *ws, int *flag) {
+    const AirPlan L = air_plan_layout(log_n, 1, 1, 0);
+    SA_TRY(coset_div_plan_build(b, plan, zerofier, zlen, log_n, root, offset, ws, flag));
+    const fe off_m = fe_to_mont(fe_from_limbs(offset));
+    SA_TRY(b.pow_table(plan + L.spw, fe_montmul(off_m, fe_to_mont(fe_from_limbs(step))), L.n));
+    SA_TRY(b.pow_table_lead(plan + L.x, fe_to_mont(fe_from_limbs(root)), off_m, L.n));
+    return b.upload(plan + L.prog, prog.data(), prog.size());
+}
+
+// The quotients of the plan's constraints for trace[nregs][ncoef] (coefficient rows): out[ncons][qlen].  The current
+// rows loaded with offset^i and the next rows with (offset * step)^j, one batched forward transform of the 2 nregs
+// rows, then per chunk of coset_batch_max(log_n) constraints k_air_eval, one batched inverse transform and the coset
+// store: 3 + 3 ceil(ncons / chunk) launches plus the transforms', whatever nregs and the chunk's size.
+// ws = air_ws_elems(nregs, ncons, log_n) elements.
+template <class B>
+int air_quotients(B &b, fe *out, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t qlen,
+                  size_t ncons, int log_n, const uint64_t root[2], fe *ws) {
+    const AirPlan L = air_plan_layout(log_n, 1, nregs, 0);
+    const long long n = L.n;
+    fe *ext = ws, *V = ws + 2 * nregs * (size_t)n;
+    SA_TRY(b.coset_load(ext, trace, plan + L.div.pw, (long long)ncoef, log_n, (long long)nregs));
+    SA_TRY(b.coset_load(ext + nregs * (size_t)n, trace, plan + L.spw, (long long)ncoef, log_n, (long long)nregs));
+    SA_TRY(b.ntt(ext, ext, log_n, root, 0, 2 * nregs));
+    const size_t chunk = air_chunk(ncons, log_n);
+    for (size_t c0 = 0; c0 < ncons; c0 += chunk) {
+        const size_t nb = std::min(chunk, ncons - c0);
+        SA_TRY(b.air_eval(V, plan + L.prog, plan + L.x, plan + L.div.inv, ext, (long long)c0, (long long)nb,
+                          (int)nregs, log_n));
+        SA_TRY(b.ntt(V, V, log_n, root, 1, nb));
+        SA_TRY(b.coset_store(out + c0 * qlen, V, plan + L.div.ipw, (long long)qlen, log_n, (long long)nb));
+    }
+    return SA_OK;
+}
+
+}  // namespace sa

@@ -1,11 +1,13 @@
 // poly.cu -- polynomial kernels: element-wise products, batch inversion, Horner evaluation, the
 // direct zerofier and Lagrange kernels, the kernels of the subproduct tree (poly_tree.cuh) behind
 // sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans, batched coset
-// evaluation and coset combinations (coset.cuh), with the backend that launches them for the headers' schedules.
+// evaluation and coset combinations (coset.cuh), and of transition quotients (air.cuh), with the backend that
+// launches them for the headers' schedules.
 //
 // Reference behaviour reproduced (bit-exact): code/ntt.py:61-176, code/algebra.py:53-57,75-94.
 #include <algorithm>
 
+#include "air.cuh"
 #include "coset.cuh"
 #include "ntt_tile.cuh"
 #include "poly_tree.cuh"
@@ -213,6 +215,11 @@ __global__ void k_coset_combine(fe *out, const __grid_constant__ CombineGroup g,
                                 int log_n, int first) {
     grid_stride(1ll << log_n, [&](long long i) { coset_combine_elem(out, g, pw_m, ncomb, first, i); });
 }
+// the quotient values of nb constraints, one thread per point
+__global__ void k_air_eval(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long c0,
+                           long long nb, int nregs, int log_n) {
+    grid_stride(1ll << log_n, [&](long long i) { air_eval_elem(V, prog, x_m, iz_m, ext, c0, nb, nregs, log_n, i); });
+}
 
 extern "C" {
 
@@ -307,6 +314,19 @@ struct DeviceTree {
     int store(fe *dst, const fe &v) {
         SA_CUDA(cudaMemcpyAsync(dst, &v, sizeof(fe), cudaMemcpyHostToDevice, st));
         return SA_OK;
+    }
+};
+// DeviceTree plus the launches only the AIR schedules make (air.cuh)
+struct DeviceAir : DeviceTree {
+    int pow_table_lead(fe *o, const fe &base_m, const fe &lead_m, ll count) {
+        return launch_pow_table(o, base_m, lead_m, count, st);
+    }
+    int upload(fe *dst, const fe *src, size_t n) {
+        SA_CUDA(cudaMemcpyAsync(dst, src, sizeof(fe) * n, cudaMemcpyHostToDevice, st));
+        return SA_OK;
+    }
+    int air_eval(fe *V, const fe *prog, const fe *x, const fe *iz, const fe *ext, ll c0, ll nb, int nregs, int lg) {
+        return go(k_air_eval, tree_grid(1ll << lg), V, prog, x, iz, ext, c0, nb, nregs, lg);
     }
 };
 static int tree_workspace(Tree &t, cudaStream_t st) {
@@ -514,6 +534,44 @@ int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], cons
     DeviceTree b{st};
     return coset_combine_evaluate(b, (fe *)out, log_n, root, offset, (const fe *const *)srcs, lens, shifts, weights,
                                   nterms, pw);
+}
+
+// ---- transition quotients (air.cuh) ----
+size_t sa_air_plan_bytes(int log_n, size_t max_ncoef, size_t nregs, size_t nterms) {
+    return sizeof(fe) * air_plan_layout(log_n, max_ncoef, nregs, nterms).elems;
+}
+
+// scratch: the zerofier's codeword (n elements, WS_AIR) and the zero flag (WS_PLAN_FLAG); the compiled program is
+// uploaded from host memory that outlives the closing synchronisation
+int sa_air_plan(void *plan, const uint64_t *coeffs, const uint32_t *exps, const size_t *term_start, size_t ncons,
+                size_t nregs, size_t max_ncoef, const void *zerofier, size_t zlen, int log_n, const uint64_t root[2],
+                const uint64_t offset[2], const uint64_t step[2], void *stream) {
+    SA_TRY(air_plan_check(log_n, exps, term_start, ncons, nregs, max_ncoef, zlen, root));
+    const std::vector<fe> prog = air_compile(coeffs, exps, term_start, ncons, nregs);
+    cudaStream_t st = (cudaStream_t)stream;
+    int *flag = nullptr;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&flag, 16, st, WS_PLAN_FLAG));
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) << log_n, st, WS_AIR));
+    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+    DeviceAir b{{st}};
+    SA_TRY(air_plan_build(b, (fe *)plan, prog, (const fe *)zerofier, zlen, log_n, root, offset, step, ws, flag));
+    int h = 0;
+    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SA_CUDA(cudaStreamSynchronize(st));
+    return h ? SA_EDIVZERO : SA_OK;
+}
+
+// Reads the plan only; its scratch is the stream's workspace (WS_AIR): 2 nregs rows of n, and n per constraint of
+// a chunk
+int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
+                     size_t ncons, int log_n, const uint64_t root[2], void *stream) {
+    SA_TRY(air_apply_check(log_n, nregs, ncoef, qlen, ncons, root));
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, ncons, log_n), st, WS_AIR));
+    DeviceAir b{{st}};
+    return air_quotients(b, (fe *)out, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons, log_n, root, ws);
 }
 
 }  // extern "C"

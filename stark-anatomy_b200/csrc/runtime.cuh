@@ -87,7 +87,8 @@ enum WsTag {
     WS_TREE = 8,           // the subproduct tree of one call (poly_tree.cuh: tree_layout)
     WS_INTERP_PLAN = 9,    // sa_interpolate's plan
     WS_INTERP_APPLY = 10,  // an apply's scratch
-    WS_COSET = 11          // coset division and evaluation (coset.cuh): the transformed rows, or offset^i
+    WS_COSET = 11,         // coset division and evaluation (coset.cuh): the transformed rows, or offset^i
+    WS_AIR = 12            // transition quotients (air.cuh): the trace's extension and a chunk's quotient rows
 };
 int get_workspace(void **out, size_t bytes, cudaStream_t st, WsTag tag);
 void keep_pool_memory();

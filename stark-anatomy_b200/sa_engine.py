@@ -66,6 +66,10 @@ SYMBOLS = [
     ("sa_coset_batch_max", _sz, [_ci]),
     ("sa_coset_combine_evaluate", _ci, [_vp, _ci, _u64p, _u64p, ctypes.POINTER(ctypes.c_void_p),
                                         ctypes.POINTER(_sz), ctypes.POINTER(_sz), _u64p, _sz, _vp]),
+    ("sa_air_plan_bytes", _sz, [_ci, _sz, _sz, _sz]),
+    ("sa_air_plan", _ci, [_vp, _u64p, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(_sz), _sz, _sz, _sz, _vp, _sz,
+                          _ci, _u64p, _u64p, _u64p, _vp]),
+    ("sa_air_quotients", _ci, [_vp, _vp, _vp, _sz, _sz, _sz, _sz, _ci, _u64p, _vp]),
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
@@ -126,6 +130,42 @@ class CosetDivPlan:
         self.log_n = log_n
         self.root = root
         self.offset = offset
+
+
+class AirPlan:
+    """A transition quotient plan (CudaEngine.air_plan): the device buffer sa_air_plan filled (torch.uint8) for one
+    AIR and zerofier on the coset offset * <root> of order 2^log_n, with the values every apply passes again"""
+    __slots__ = ("plan", "log_n", "root", "offset", "nregs", "ncons", "max_ncoef")
+
+    def __init__(self, plan, log_n, root, offset, nregs, ncons, max_ncoef):
+        self.plan = plan
+        self.log_n = log_n
+        self.root = root
+        self.offset = offset
+        self.nregs = nregs
+        self.ncons = ncons
+        self.max_ncoef = max_ncoef
+
+
+def _air_arrays(constraints, nregs):
+    """the C ABI's coefficient limbs, exponents and term_start of constraints given as objects with a `.dictionary`
+    (MPolynomial) or as {exponent tuple: value} dicts, values ints or anything with `.value`; tuples shorter than
+    1 + 2 nregs are zero-padded (as MPolynomial.__add__ pads) and terms that meet there are added"""
+    nvars = 1 + 2 * nregs
+    coeffs, exps, starts = [], [], [0]
+    for a in constraints:
+        terms = {}
+        for k, v in getattr(a, "dictionary", a).items():
+            k = tuple(int(e) for e in k)
+            if len(k) > nvars or any(not 0 <= e < 1 << 32 for e in k):
+                raise SaError(SA_ERRORS[-6])
+            k += (0,) * (nvars - len(k))
+            terms[k] = (terms.get(k, 0) + int(getattr(v, "value", v))) % P
+        for k, v in terms.items():
+            coeffs += [v & 0xFFFFFFFFFFFFFFFF, v >> 64]
+            exps += k
+        starts.append(len(exps) // nvars)
+    return coeffs, exps, starts
 
 
 class CudaEngine:
@@ -386,6 +426,50 @@ class CudaEngine:
             out.data_ptr(), log_n, _limbs(root), _limbs(offset), (ctypes.c_void_p * t)(*ptrs),
             (ctypes.c_size_t * t)(*lens), (ctypes.c_size_t * t)(*shifts), (ctypes.c_uint64 * (2 * t))(*weights), t,
             self._stream()))
+        return out
+
+    def air_plan(self, constraints, nregs, zerofier, max_ncoef, log_n, root, offset, step):
+        """sa_air_plan: the transition constraints (MPolynomials or {exponent tuple: value} dicts over x, the nregs
+        trace rows and the nregs next rows T(step * x)) compiled with the zerofier's (zlen, 2) coset division plan on
+        the coset offset * <root> of order 2^log_n, for trace polynomials of up to max_ncoef coefficients
+        (synchronises; "unsupported size" when a term's degree bound reaches n, "divide by zero" when the zerofier
+        vanishes on the coset)"""
+        nregs, max_ncoef = int(nregs), int(max_ncoef)
+        constraints = list(constraints)
+        if nregs < 1 or not constraints or zerofier.dim() != 2:
+            raise SaError(SA_ERRORS[-6])
+        if self.lib.sa_air_plan_bytes(log_n, max_ncoef, nregs, 0) == 0:
+            raise SaError(SA_ERRORS[-6])
+        self._rows(zerofier, 1 << log_n)
+        coeffs, exps, starts = _air_arrays(constraints, nregs)
+        nbytes = self.lib.sa_air_plan_bytes(log_n, max_ncoef, nregs, starts[-1])
+        if nbytes == 0:
+            raise SaError(SA_ERRORS[-6])
+        zerofier = zerofier.contiguous()
+        plan = self.torch.empty(nbytes, dtype=self.torch.uint8, device=self.device)
+        ncons = len(constraints)
+        self._check(self.lib.sa_air_plan(
+            plan.data_ptr(), (ctypes.c_uint64 * max(len(coeffs), 1))(*coeffs),
+            (ctypes.c_uint32 * max(len(exps), 1))(*exps), (ctypes.c_size_t * (ncons + 1))(*starts), ncons, nregs,
+            max_ncoef, zerofier.data_ptr(), zerofier.shape[0], log_n, _limbs(root), _limbs(offset), _limbs(step),
+            self._stream()))
+        return AirPlan(plan, log_n, int(root), int(offset), nregs, ncons, max_ncoef)
+
+    def air_quotients(self, plan, trace, qlen):
+        """sa_air_quotients: the first qlen coefficients of every constraint's quotient for the trace polynomials
+        (nregs, ncoef, 2), ncoef <= the plan's max_ncoef -> (ncons, qlen, 2), in one call; asynchronous, the plan is
+        only read"""
+        torch = self.torch
+        # the library cannot see the tensor's shape, dtype or device
+        if (not isinstance(trace, torch.Tensor) or trace.dtype != torch.int64 or trace.device != self.device
+                or trace.dim() != 3 or trace.shape[0] != plan.nregs or trace.shape[2] != 2
+                or not 1 <= trace.shape[1] <= plan.max_ncoef or not 1 <= int(qlen) <= 1 << plan.log_n):
+            raise SaError(SA_ERRORS[-6])
+        trace = trace.contiguous()
+        out = torch.empty((plan.ncons, int(qlen), 2), dtype=torch.int64, device=self.device)
+        self._check(self.lib.sa_air_quotients(out.data_ptr(), plan.plan.data_ptr(), trace.data_ptr(), plan.nregs,
+                                              trace.shape[1], int(qlen), plan.ncons, plan.log_n, _limbs(plan.root),
+                                              self._stream()))
         return out
 
     # --------------------------------------------------------------- merkle
