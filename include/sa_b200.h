@@ -276,6 +276,40 @@ int sa_air_plan(void *plan, const uint64_t *coeffs, const uint32_t *exps, const 
 int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
                      size_t ncons, int log_n, const uint64_t root[2], void *stream);
 
+/* ---- code/fast_stark.py:92-106: the boundary quotients, their coset codewords and a remainder check ------------
+ * Register s has the trace polynomial T_s, the interpolant I_s of its boundary values and the zerofier Z_s of its
+ * boundary points.  With n = 2^log_n and x_i = offset * root^i (FastStark's FRI domain: offset = the generator,
+ * root = omega) an apply gives
+ *     codewords[s][i] = (T_s(x_i) - I_s(x_i)) / Z_s(x_i),   quot[s][j] = U_s[j] * offset^-j (j < ncoef),
+ * U_s = intt(codewords[s]), and flags[s] = 0 exactly when (T_s - I_s) / Z_s is a clean division: when U_s is zero at
+ * every j >= max(0, ncoef - deg Z_s).  Then quot[s] is the reference's quotient followed by zeros and codewords[s] is
+ * fast_coset_evaluate's of it, bit for bit; otherwise the reference raises "cannot perform polynomial division because
+ * remainder is not zero" and the row is not a quotient.
+ * A plan holds offset^i, offset^-i and per register 1/Z_s(x_i), I_s(x_i) and deg Z_s.  It is a device buffer the
+ * caller owns, of sa_boundary_plan_bytes(log_n, nregs) bytes: 32*n*(1 + nregs) + 16*sec16(nregs) from n = 16 on,
+ * sec16 rounding up to a multiple of 16 (DESIGN section 2).  0 when log_n is outside 1..30, nregs == 0 or the size
+ * does not fit a size_t.  Host-only: no CUDA call.                                                                  */
+size_t sa_boundary_plan_bytes(int log_n, size_t nregs);
+/* Builds the plan from per-register device rows zerofiers[s][0..zlens[s]) and interpolants[s][0..ilens[s]); the
+ * pointer and length arrays are HOST arrays.  Before any launch: SA_ESIZE for log_n outside 1..30, nregs == 0, a
+ * zlens[s] or ilens[s] outside 1..n, and offset 0 (the check needs n distinct points); the root's SA_EROOTORDER /
+ * SA_ENOTPRIM.  After the build's one synchronisation: SA_ESIZE when a zerofier row's top coefficient is zero (deg Z_s
+ * is taken as zlens[s] - 1), else SA_EDIVZERO when some Z_s vanishes on the coset.                                  */
+int sa_boundary_plan(void *plan, const void *const *zerofiers, const size_t *zlens, const void *const *interpolants,
+                     const size_t *ilens, size_t nregs, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                     void *stream);
+/* quot[nregs][ncoef], codewords[nregs][n] and flags[nregs] (above) from trace[nregs][ncoef], the trace polynomials'
+ * coefficient rows (sa_interp_apply_batch's layout).  log_n, root and nregs must be the plan's.  SA_ESIZE before any
+ * launch for nregs == 0 or ncoef outside 1..n.  Rows are contiguous, so they feed sa_coset_combine_evaluate and
+ * sa_coset_evaluate_batch as they are.  Launches: a memset that clears the flags, then per chunk of
+ * sa_coset_batch_max(log_n) registers the coset load, one batched forward sa_ntt in the codewords, the point kernel,
+ * one batched inverse sa_ntt into the workspace and the store with the remainder check -- the same count whatever the
+ * chunk's size.  Per-stream workspace: 16*n bytes per register of a chunk besides the transform's.  Asynchronous: no
+ * host synchronisation, and no allocation once the stream's workspaces have grown, so the call can be captured in a
+ * CUDA graph; a replay clears the flags again.  Reads the plan only: one plan may be applied on several streams.   */
+int sa_boundary_quotients(void *quot, void *codewords, uint32_t *flags, const void *plan, const void *trace,
+                          size_t nregs, size_t ncoef, int log_n, const uint64_t root[2], void *stream);
+
 /* ---- code/merkle.py:6-14 Merkle.commit -------------------------------------------------
  * Builds the whole blake2b-512 tree over n = 2^k leaves, leaf = H(decimal ASCII of the
  * value), node = H(left || right).  `tree` receives 2n nodes of 64 bytes in heap order:

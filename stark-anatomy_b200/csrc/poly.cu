@@ -1,13 +1,14 @@
 // poly.cu -- polynomial kernels: element-wise products, batch inversion, Horner evaluation, the
 // direct zerofier and Lagrange kernels, the kernels of the subproduct tree (poly_tree.cuh) behind
 // sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans, batched coset
-// evaluation and coset combinations (coset.cuh), and of transition quotients (air.cuh), with the backend that
-// launches them for the headers' schedules.
+// evaluation and coset combinations (coset.cuh), of transition quotients (air.cuh) and of boundary quotients
+// (boundary.cuh), with the backend that launches them for the headers' schedules.
 //
 // Reference behaviour reproduced (bit-exact): code/ntt.py:61-176, code/algebra.py:53-57,75-94.
 #include <algorithm>
 
 #include "air.cuh"
+#include "boundary.cuh"
 #include "coset.cuh"
 #include "ntt_tile.cuh"
 #include "poly_tree.cuh"
@@ -220,6 +221,22 @@ __global__ void k_air_eval(fe *V, const fe *prog, const fe *x_m, const fe *iz_m,
                            long long nb, int nregs, int log_n) {
     grid_stride(1ll << log_n, [&](long long i) { air_eval_elem(V, prog, x_m, iz_m, ext, c0, nb, nregs, log_n, i); });
 }
+// the boundary quotient codewords of batch registers in place, one thread per point
+__global__ void k_boundary_point(fe *cw, const fe *ival, const fe *izinv_m, long long stride, int log_n,
+                                 long long batch) {
+    grid_stride(batch << log_n, [&](long long idx) { boundary_point_elem(cw, ival, izinv_m, stride, log_n, idx); });
+}
+// the quotient rows of batch registers and their remainder flags: every lane of a warp runs the same iterations (the
+// range is rounded up to whole warps), so the ballot is over the full warp and each row a warp touches costs one
+// atomicOr at most
+__global__ void k_boundary_store(fe *quot, uint32_t *flags, const fe *ws, const fe *ipw_m, const fe *deg,
+                                 long long ncoef, int log_n, long long batch) {
+    grid_stride(((batch << log_n) + 31) & ~31ll, [&](long long idx) {
+        const bool bad = boundary_store_elem(quot, ws, ipw_m, deg, ncoef, log_n, batch, idx);
+        const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, bad);
+        if (bad && boundary_flag_leader(ballot, threadIdx.x & 31, log_n)) atomicOr(flags + (idx >> log_n), 1u);
+    });
+}
 
 extern "C" {
 
@@ -327,6 +344,23 @@ struct DeviceAir : DeviceTree {
     }
     int air_eval(fe *V, const fe *prog, const fe *x, const fe *iz, const fe *ext, ll c0, ll nb, int nregs, int lg) {
         return go(k_air_eval, tree_grid(1ll << lg), V, prog, x, iz, ext, c0, nb, nregs, lg);
+    }
+};
+// DeviceAir (its upload) plus the copies and launches only the boundary schedules make (boundary.cuh)
+struct DeviceBoundary : DeviceAir {
+    int download(fe *dst, const fe *src, size_t n) {
+        SA_CUDA(cudaMemcpyAsync(dst, src, sizeof(fe) * n, cudaMemcpyDeviceToHost, st));
+        return SA_OK;
+    }
+    int clear_flags(uint32_t *flags, size_t n) {
+        SA_CUDA(cudaMemsetAsync(flags, 0, sizeof(uint32_t) * n, st));
+        return SA_OK;
+    }
+    int boundary_point(fe *cw, const fe *iv, const fe *iz, ll stride, int lg, ll nb) {
+        return go(k_boundary_point, tree_grid(nb << lg), cw, iv, iz, stride, lg, nb);
+    }
+    int boundary_store(fe *q, uint32_t *flags, const fe *ws, const fe *ipw, const fe *deg, ll nc, int lg, ll nb) {
+        return go(k_boundary_store, tree_grid(nb << lg), q, flags, ws, ipw, deg, nc, lg, nb);
     }
 };
 static int tree_workspace(Tree &t, cudaStream_t st) {
@@ -572,6 +606,46 @@ int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nreg
     SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, ncons, log_n), st, WS_AIR));
     DeviceAir b{{st}};
     return air_quotients(b, (fe *)out, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons, log_n, root, ws);
+}
+
+// ---- boundary quotients (boundary.cuh) ----
+size_t sa_boundary_plan_bytes(int log_n, size_t nregs) {
+    return sizeof(fe) * boundary_plan_layout(log_n, nregs).elems;
+}
+
+// scratch: one register's zerofier codeword at a time (n elements, WS_COSET) and the zero flag (WS_PLAN_FLAG); the
+// top coefficients and the degrees go through host memory that outlives the closing synchronisation
+int sa_boundary_plan(void *plan, const void *const *zerofiers, const size_t *zlens, const void *const *interpolants,
+                     const size_t *ilens, size_t nregs, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                     void *stream) {
+    SA_TRY(boundary_plan_check(log_n, zlens, ilens, nregs, root, offset));
+    cudaStream_t st = (cudaStream_t)stream;
+    int *flag = nullptr;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&flag, 16, st, WS_PLAN_FLAG));
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) << log_n, st, WS_COSET));
+    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+    std::vector<fe> tops(nregs), degs(nregs);
+    DeviceBoundary b{{{st}}};
+    SA_TRY(boundary_plan_build(b, (fe *)plan, (const fe *const *)zerofiers, zlens, (const fe *const *)interpolants,
+                               ilens, nregs, log_n, root, offset, ws, flag, tops.data(), degs.data()));
+    int h = 0;
+    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SA_CUDA(cudaStreamSynchronize(st));
+    return boundary_plan_verdict(tops.data(), nregs, h);
+}
+
+// Reads the plan only; its scratch is the stream's workspace (WS_COSET): n elements per register of a chunk
+int sa_boundary_quotients(void *quot, void *codewords, uint32_t *flags, const void *plan, const void *trace,
+                          size_t nregs, size_t ncoef, int log_n, const uint64_t root[2], void *stream) {
+    SA_TRY(boundary_apply_check(log_n, nregs, ncoef, root));
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *ws = nullptr;
+    const size_t chunk = std::min(nregs, coset_batch_max(log_n));
+    SA_TRY(get_workspace((void **)&ws, (sizeof(fe) << log_n) * chunk, st, WS_COSET));
+    DeviceBoundary b{{{st}}};
+    return boundary_quotients(b, (fe *)quot, (fe *)codewords, flags, (const fe *)plan, (const fe *)trace, nregs, ncoef,
+                              log_n, root, ws);
 }
 
 }  // extern "C"

@@ -70,6 +70,10 @@ SYMBOLS = [
     ("sa_air_plan", _ci, [_vp, _u64p, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(_sz), _sz, _sz, _sz, _vp, _sz,
                           _ci, _u64p, _u64p, _u64p, _vp]),
     ("sa_air_quotients", _ci, [_vp, _vp, _vp, _sz, _sz, _sz, _sz, _ci, _u64p, _vp]),
+    ("sa_boundary_plan_bytes", _sz, [_ci, _sz]),
+    ("sa_boundary_plan", _ci, [_vp, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_sz),
+                               ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_sz), _sz, _ci, _u64p, _u64p, _vp]),
+    ("sa_boundary_quotients", _ci, [_vp, _vp, ctypes.POINTER(ctypes.c_uint32), _vp, _vp, _sz, _sz, _ci, _u64p, _vp]),
     ("sa_merkle_tree", _ci, [_vp, _vp, _sz, _vp]),
     ("sa_merkle_open", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
     ("sa_gather", _ci, [_vp, _vp, _sz, _u64p, _sz, _vp]),
@@ -145,6 +149,28 @@ class AirPlan:
         self.nregs = nregs
         self.ncons = ncons
         self.max_ncoef = max_ncoef
+
+
+class BoundaryPlan:
+    """A boundary quotient plan (CudaEngine.boundary_plan): the device buffer sa_boundary_plan filled (torch.uint8)
+    for one boundary on the coset offset * <root> of order 2^log_n, with the values every apply passes again and the
+    degree of each register's boundary zerofier (its number of boundary points)"""
+    __slots__ = ("plan", "log_n", "root", "offset", "nregs", "degrees")
+
+    def __init__(self, plan, log_n, root, offset, nregs, degrees):
+        self.plan = plan
+        self.log_n = log_n
+        self.root = root
+        self.offset = offset
+        self.nregs = nregs
+        self.degrees = degrees
+
+    def degree_bounds(self, trace_length):
+        """FastStark.boundary_quotient_degree_bounds for trace polynomials of trace_length coefficients"""
+        return [trace_length - 1 - d for d in self.degrees]
+
+
+REMAINDER = "cannot perform polynomial division because remainder is not zero"  # univariate.py:52
 
 
 def _air_arrays(constraints, nregs):
@@ -471,6 +497,70 @@ class CudaEngine:
                                               trace.shape[1], int(qlen), plan.ncons, plan.log_n, _limbs(plan.root),
                                               self._stream()))
         return out
+
+    def _ints(self, values):
+        """a list of ints -> device vector (n, 2)"""
+        return self.upload(bytearray(b"".join((int(v) % P).to_bytes(16, "little") for v in values)))
+
+    def boundary_plan(self, boundary, nregs, omicron, log_n, root, offset):
+        """sa_boundary_plan: for FastStark's boundary, a list of (cycle, register, value) with values ints or
+        FieldElements, register s's points omicron^cycle, its zerofier Z_s (`zerofier`) and interpolant I_s
+        (`interpolate`) on the device, planned on the coset offset * <root> of order 2^log_n (synchronises).
+        "unsupported size" before any device work for offset 0, a register outside 0..nregs-1, a register without
+        boundary points (the reference's interpolate_domain refuses those) or one with n or more; "divide by zero"
+        when two of a register's cycles give one point, or when a zerofier vanishes on the coset"""
+        nregs = int(nregs)
+        if nregs < 1 or self.lib.sa_boundary_plan_bytes(log_n, nregs) == 0 or int(offset) % P == 0:
+            raise SaError(SA_ERRORS[-6])
+        w = int(getattr(omicron, "value", omicron))
+        points = [[] for _ in range(nregs)]
+        for c, r, v in boundary:
+            if not 0 <= int(r) < nregs:
+                raise SaError(SA_ERRORS[-6])
+            points[int(r)].append((pow(w, int(c), P), int(getattr(v, "value", v))))
+        if any(not 1 <= len(pts) < 1 << log_n for pts in points):
+            raise SaError(SA_ERRORS[-6])
+        zs, its = [], []
+        for pts in points:
+            domain = self._ints([x for x, _ in pts])
+            its.append(self.interpolate(domain, self._ints([v for _, v in pts])))
+            zs.append(self.zerofier(domain))
+        plan = self.torch.empty(self.lib.sa_boundary_plan_bytes(log_n, nregs), dtype=self.torch.uint8,
+                                device=self.device)
+        vp, sz = ctypes.c_void_p * nregs, ctypes.c_size_t * nregs
+        self._check(self.lib.sa_boundary_plan(
+            plan.data_ptr(), vp(*[z.data_ptr() for z in zs]), sz(*[z.shape[0] for z in zs]),
+            vp(*[i.data_ptr() for i in its]), sz(*[i.shape[0] for i in its]), nregs, log_n, _limbs(root),
+            _limbs(int(offset) % P), self._stream()))
+        return BoundaryPlan(plan, log_n, int(root), int(offset) % P, nregs, [len(pts) for pts in points])
+
+    def boundary_quotients(self, plan, trace, check=True):
+        """sa_boundary_quotients: for the trace polynomials (nregs, ncoef, 2), each register's boundary quotient
+        (T_s - I_s) / Z_s followed by zeros (nregs, ncoef, 2), its codeword on the plan's coset (nregs, n, 2) and the
+        remainder flags (nregs,) int32, non-zero where the division is not clean.  check=True reads the flags (one
+        synchronisation) and raises the reference's remainder message naming the registers; check=False stays
+        asynchronous.  The plan is only read."""
+        torch = self.torch
+        n = 1 << plan.log_n
+        # the library cannot see the tensor's shape, dtype or device
+        if (not isinstance(trace, torch.Tensor) or trace.dtype != torch.int64 or trace.device != self.device
+                or trace.dim() != 3 or trace.shape[0] != plan.nregs or trace.shape[2] != 2
+                or not 1 <= trace.shape[1] <= n):
+            raise SaError(SA_ERRORS[-6])
+        trace = trace.contiguous()
+        ncoef = trace.shape[1]
+        quot = torch.empty((plan.nregs, ncoef, 2), dtype=torch.int64, device=self.device)
+        codewords = torch.empty((plan.nregs, n, 2), dtype=torch.int64, device=self.device)
+        flags = torch.empty(plan.nregs, dtype=torch.int32, device=self.device)
+        self._check(self.lib.sa_boundary_quotients(
+            quot.data_ptr(), codewords.data_ptr(), ctypes.cast(flags.data_ptr(), ctypes.POINTER(ctypes.c_uint32)),
+            plan.plan.data_ptr(), trace.data_ptr(), plan.nregs, ncoef, plan.log_n, _limbs(plan.root), self._stream()))
+        if check:
+            self._count("d2h", 4 * plan.nregs)
+            bad = [s for s, f in enumerate(flags.tolist()) if f]
+            if bad:
+                raise SaError("%s (registers %s)" % (REMAINDER, bad))
+        return quot, codewords, flags
 
     # --------------------------------------------------------------- merkle
     def _new_tree(self, n):
