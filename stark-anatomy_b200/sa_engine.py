@@ -411,15 +411,27 @@ class CudaEngine:
                                                           self._stream()))
         return out
 
-    def coset_evaluate(self, coeffs, log_n, root, offset):
+    def _out(self, out, shape):
+        """a caller's output buffer: a contiguous int64 tensor of exactly `shape` on this device (a row range of a
+        larger buffer qualifies); a new tensor when out is None"""
+        torch = self.torch
+        if out is None:
+            return torch.empty(shape, dtype=torch.int64, device=self.device)
+        if (not isinstance(out, torch.Tensor) or out.dtype != torch.int64 or out.device != self.device
+                or tuple(out.shape) != tuple(shape) or not out.is_contiguous()):
+            raise SaError(SA_ERRORS[-6])
+        return out
+
+    def coset_evaluate(self, coeffs, log_n, root, offset, out=None):
         """sa_coset_evaluate_batch: fast_coset_evaluate at order 2^log_n of one polynomial (ncoef, 2) -> (n, 2) or of
-        a batch (B, ncoef, 2) -> (B, n, 2) in one call; asynchronous"""
+        a batch (B, ncoef, 2) -> (B, n, 2) in one call; asynchronous.  `out`, when given, is the contiguous (n, 2) /
+        (B, n, 2) tensor the values are written to (and returned)"""
         if self.lib.sa_coset_batch_max(log_n) == 0:
             raise SaError(SA_ERRORS[-6])
         n = 1 << log_n
         batch = self._rows(coeffs, n)
         coeffs = coeffs.contiguous()
-        out = self.torch.empty(tuple(coeffs.shape[:-2]) + (n, 2), dtype=self.torch.int64, device=self.device)
+        out = self._out(out, tuple(coeffs.shape[:-2]) + (n, 2))
         if batch:
             self._check(self.lib.sa_coset_evaluate_batch(out.data_ptr(), coeffs.data_ptr(), coeffs.shape[-2], log_n,
                                                          _limbs(root), _limbs(offset), batch, self._stream()))
@@ -534,12 +546,13 @@ class CudaEngine:
             _limbs(int(offset) % P), self._stream()))
         return BoundaryPlan(plan, log_n, int(root), int(offset) % P, nregs, [len(pts) for pts in points])
 
-    def boundary_quotients(self, plan, trace, check=True):
+    def boundary_quotients(self, plan, trace, check=True, out=None):
         """sa_boundary_quotients: for the trace polynomials (nregs, ncoef, 2), each register's boundary quotient
         (T_s - I_s) / Z_s followed by zeros (nregs, ncoef, 2), its codeword on the plan's coset (nregs, n, 2) and the
         remainder flags (nregs,) int32, non-zero where the division is not clean.  check=True reads the flags (one
         synchronisation) and raises the reference's remainder message naming the registers; check=False stays
-        asynchronous.  The plan is only read."""
+        asynchronous.  `out`, when given, is the contiguous (nregs, n, 2) tensor the codewords are written to (and
+        returned), e.g. the first rows of a buffer that more codewords share.  The plan is only read."""
         torch = self.torch
         n = 1 << plan.log_n
         # the library cannot see the tensor's shape, dtype or device
@@ -550,7 +563,7 @@ class CudaEngine:
         trace = trace.contiguous()
         ncoef = trace.shape[1]
         quot = torch.empty((plan.nregs, ncoef, 2), dtype=torch.int64, device=self.device)
-        codewords = torch.empty((plan.nregs, n, 2), dtype=torch.int64, device=self.device)
+        codewords = self._out(out, (plan.nregs, n, 2))
         flags = torch.empty(plan.nregs, dtype=torch.int32, device=self.device)
         self._check(self.lib.sa_boundary_quotients(
             quot.data_ptr(), codewords.data_ptr(), ctypes.cast(flags.data_ptr(), ctypes.POINTER(ctypes.c_uint32)),

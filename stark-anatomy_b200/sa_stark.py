@@ -1,0 +1,354 @@
+"""sa_stark -- FastStark.prove on the device: from the trace to the serialized proof through the planned stages.
+
+The reference's prover (code/fast_stark.py:76-178) interpolates the trace, divides out the boundary and the
+transition zerofiers, commits, combines and runs FRI in Python.  ``StarkPlan.prove`` runs the same schedule through
+the engine's planned calls, and only roots, challenges and opened leaves cross to the host:
+
+  1. the trace randomizers are drawn with the caller's ``field.sample(os.urandom(17))``, in the reference's order;
+  2. the columns are packed and uploaded once, and one batched ``interp_apply`` gives the trace polynomials;
+  3. ``boundary_quotients`` gives each register's quotient and codeword, and raises the reference's remainder
+     message when a boundary value is false;
+  4. ``air_quotients`` divides every transition constraint at the order the reference divides it at (one AIR plan
+     per order), and the divisions the reference refuses are refused with its messages;
+  5. the randomizer polynomial is drawn where the reference draws it, its codeword is written next to the boundary
+     codewords, and one ``merkle_trees`` call commits all of them;
+  6. the weights come from the caller's ``prover_fiat_shamir()``; the degree check reads one coefficient per
+     constraint; one ``coset_combine_evaluate`` gives the combined codeword;
+  7. the drop-in ``Fri.prove`` runs on that codeword where it lies;
+  8. the openings are one gather and one path read for the boundary and randomizer codewords, and the zerofier
+     codeword's own.
+
+The proof bytes are the reference's (DESIGN section 3.9 gives the argument), or an AssertionError: inputs this
+schedule cannot decide exactly are refused rather than proven differently.
+
+``enable(cls)`` rebinds ``cls.prove`` (FastStark's) to ``prove``; ``disable()`` restores it.  Off by default, as
+``sa_accel``.  Nothing here imports torch or holds device state outside a ``StarkPlan``.
+"""
+import os
+from hashlib import blake2b
+
+import sa_host
+import sa_engine
+import sa_devlist
+import sa_marshal
+import fri as _fri
+
+P = sa_engine.P
+FieldElement = sa_host.algebra.FieldElement
+REMAINDER = sa_engine.REMAINDER
+DEGREE_MISMATCH = "transition quotient degrees do not match with expectation"      # fast_stark.py:127
+LARGER_DEGREE = "cannot divide by polynomial of larger degree"                     # ntt.py:145
+ZERO_DIVISOR = "cannot divide by zero polynomial"                                  # ntt.py:140
+LONG_DIVISION_BELOW = 8  # ntt.py:152: below this degree the reference divides by long division
+
+
+def _bits(x):
+    """the number of binary digits FastStark counts for x: len(bin(x)) without its two-character prefix"""
+    return max(1, x.bit_length()) if x >= 0 else x.bit_length() + 1
+
+
+def _terms(constraint):
+    """a constraint's (exponent tuple, int coefficient) pairs, from an MPolynomial or an {exponent tuple: value}
+    dict, with zero coefficients kept (FastStark's degree bounds count them)"""
+    return [(tuple(int(e) for e in k), int(getattr(v, "value", v)) % P)
+            for k, v in getattr(constraint, "dictionary", constraint).items()]
+
+
+def _term_degree(k, trace_degree):
+    """degree of a term's numerator with x of degree 1 and every trace row of degree trace_degree"""
+    return sum(e * (1 if i == 0 else trace_degree) for i, e in enumerate(k))
+
+
+def _ints(values):
+    return [int(getattr(v, "value", v)) for v in values]
+
+
+def _value(lo, hi):
+    """the residue of one element's two 64-bit limbs (signed or unsigned, as the engine returns them)"""
+    return (int(lo) & 0xFFFFFFFFFFFFFFFF) | (int(hi) & 0xFFFFFFFFFFFFFFFF) << 64
+
+
+def _degree(values):
+    d = -1
+    for i, v in enumerate(values):
+        if v:
+            d = i
+    return d
+
+
+class Params:
+    """What FastStark.__init__ derives from its arguments, with its degree bounds and weight sampling, restated from
+    the reference's behaviour so that a prove needs no reference checkout; ``fri`` is a drop-in ``fri.Fri``."""
+
+    def __init__(self, field, expansion_factor, num_colinearity_checks, security_level, num_registers, num_cycles,
+                 transition_constraints_degree=2):
+        assert len(bin(field.p)) - 2 >= security_level, "p must have at least as many bits as security level"
+        assert expansion_factor & (expansion_factor - 1) == 0, "expansion factor must be a power of 2"
+        assert expansion_factor >= 4, "expansion factor must be 4 or greater"
+        assert num_colinearity_checks * 2 >= security_level, \
+            "number of colinearity checks must be at least half of security level"
+        self.field = field
+        self.expansion_factor = expansion_factor
+        self.num_colinearity_checks = num_colinearity_checks
+        self.security_level = security_level
+        self.num_randomizers = 4 * num_colinearity_checks
+        self.num_registers = num_registers
+        self.original_trace_length = num_cycles
+        self.randomized_trace_length = num_cycles + self.num_randomizers
+        self.omicron_domain_length = 1 << _bits(self.randomized_trace_length * transition_constraints_degree)
+        self.fri_domain_length = self.omicron_domain_length * expansion_factor
+        self.generator = field.generator()
+        self.omega = field.primitive_nth_root(self.fri_domain_length)
+        self.omicron = field.primitive_nth_root(self.omicron_domain_length)
+        self.fri = _fri.Fri(self.generator, self.omega, self.fri_domain_length, expansion_factor,
+                            num_colinearity_checks)
+
+    def transition_degree_bounds(self, transition_constraints):
+        trace_degree = self.original_trace_length + self.num_randomizers - 1
+        return [max(_term_degree(k[:1 + 2 * self.num_registers], trace_degree) for k, _ in _terms(a))
+                for a in transition_constraints]
+
+    def transition_quotient_degree_bounds(self, transition_constraints):
+        return [d - (self.original_trace_length - 1) for d in self.transition_degree_bounds(transition_constraints)]
+
+    def max_degree(self, transition_constraints):
+        return (1 << _bits(max(self.transition_quotient_degree_bounds(transition_constraints)))) - 1
+
+    def boundary_quotient_degree_bounds(self, randomized_trace_length, boundary):
+        """randomized_trace_length - 1 minus each register's number of boundary points (its zerofier's degree)"""
+        if any(all(r != s for _, r, _ in boundary) for s in range(self.num_registers)):
+            raise IndexError("list index out of range")  # the reference's zerofier_domain of no points
+        return [randomized_trace_length - 1 - sum(1 for _, r, _ in boundary if r == s)
+                for s in range(self.num_registers)]
+
+    def sample_weights(self, number, randomness):
+        return [self.field.sample(blake2b(randomness + bytes(i)).digest()) for i in range(number)]
+
+
+class _Constraint:
+    __slots__ = ("index", "degree", "bound", "top", "kind", "order")
+
+
+class StarkPlan:
+    """What does not change between proofs of one AIR on one FastStark (or ``Params``): the interpolation plan of
+    the randomized trace domain, one AIR plan per division order with the zerofier uploaded once, and the
+    constraints' degrees, bounds and shifts.  Only read by ``prove``."""
+
+    def __init__(self, stark, transition_constraints, transition_zerofier):
+        eng = sa_engine.get_engine()
+        self.stark = stark
+        field = stark.field
+        nregs = stark.num_registers
+        self.nregs = nregs
+        self.ncycles = stark.original_trace_length
+        self.trace_length = self.ncycles + stark.num_randomizers
+        odl, n = stark.omicron_domain_length, stark.fri_domain_length
+        self.log_n = n.bit_length() - 1
+        omicron = stark.omicron.value
+        T = self.trace_length
+
+        fri = getattr(stark, "fri", None)
+        self.fri = fri if isinstance(fri, _fri.Fri) else _fri.Fri(
+            stark.generator, stark.omega, n, stark.expansion_factor, stark.num_colinearity_checks)
+
+        zerofier = _ints(getattr(transition_zerofier, "coefficients", transition_zerofier))
+        zdeg = _degree(zerofier)
+        assert zdeg >= 0, ZERO_DIVISOR
+        # the bounds subtract original_trace_length - 1 where the quotients' lengths subtract deg Z: the two agree
+        # only for the zerofier FastStark.preprocess builds
+        assert zdeg == self.ncycles - 1, \
+            "sa_stark: the transition zerofier has degree %d, not original_trace_length - 1 = %d" % (zdeg, self.ncycles - 1)
+
+        self.constraints = list(transition_constraints)
+        self.cons = []
+        for c, a in enumerate(self.constraints):
+            terms = [(k, v) for k, v in _terms(a)]
+            if any(len(k) > 1 + 2 * nregs for k, _ in terms):
+                raise AssertionError(sa_engine.SA_ERRORS[-6])
+            k = _Constraint()
+            k.index = c
+            degs = [_term_degree(e, T - 1) for e, _ in terms]
+            k.degree = max(degs)  # ValueError for a constraint without terms, as the reference's max()
+            k.bound = k.degree - (self.ncycles - 1)
+            k.top = [(e, v) for (e, v), d in zip(terms, degs) if d == k.degree]
+            if k.degree < zdeg:
+                k.kind, k.order = "larger", None
+            elif k.degree < LONG_DIVISION_BELOW:
+                # long division in the reference: a clean quotient is the coset quotient at any order above the
+                # degree; the whole row is read to check the division is clean
+                k.kind, k.order = "long", 1 << max(_bits(k.degree), (T - 1).bit_length())
+            else:
+                assert k.degree < odl, "sa_stark: transition constraint %d has degree %d, at or above the omicron " \
+                    "domain's length %d (the reference's transform aliases there)" % (c, k.degree, odl)
+                order = odl
+                while k.degree < order // 2:
+                    order //= 2
+                assert order >= T, "sa_stark: transition constraint %d divides at order %d, below the randomized " \
+                    "trace length %d" % (c, order, T)
+                k.kind, k.order = "transform", order
+            self.cons.append(k)
+        bounds = [k.bound for k in self.cons]
+        self.max_degree = (1 << _bits(max(bounds))) - 1
+
+        # one AIR plan per division order, the zerofier uploaded once
+        self.zerofier = eng.upload(sa_devlist.pack([FieldElement(v, field) for v in zerofier[:zdeg + 1]]))
+        self.groups = []  # (order, AirPlan, constraint indices, qlen)
+        for order in sorted({k.order for k in self.cons if k.order is not None}):
+            idx = [k.index for k in self.cons if k.order == order]
+            long = self.cons[idx[0]].kind == "long"
+            plan = eng.air_plan([self.constraints[c] for c in idx], nregs, self.zerofier, T, order.bit_length() - 1,
+                                pow(omicron, odl // order, P), stark.generator.value, omicron)
+            self.groups.append((order, plan, idx, order if long else max(self.cons[c].bound for c in idx) + 1))
+
+        domain = [FieldElement(pow(omicron, i, P), field) for i in range(T)]
+        self.interp = eng.interp_plan(eng.upload(sa_devlist.pack(domain)))
+
+    def _top_coefficient(self, k, tops):
+        """the coefficient of x^degree in constraint k's numerator: its maximal-degree terms on the trace
+        polynomials' top coefficients (a next-row variable's top coefficient carries omicron^(T - 1))"""
+        nregs = self.nregs
+        shift = pow(self.stark.omicron.value, self.trace_length - 1, P)
+        acc = 0
+        for e, v in k.top:
+            t = v
+            for i, x in enumerate(e[1:]):
+                if x:
+                    top = tops[i] if i < nregs else tops[i - nregs] * shift % P
+                    t = t * pow(top, x, P) % P
+            acc += t
+        return acc % P
+
+    def prove(self, trace, boundary, transition_zerofier_codeword, proof_stream=None):
+        """FastStark.prove(trace, constraints, boundary, zerofier, zerofier_codeword, proof_stream) for this plan's
+        constraints and zerofier: proof_stream.serialize()"""
+        eng = sa_engine.get_engine()
+        stark = self.stark
+        field = stark.field
+        nregs, T, log_n = self.nregs, self.trace_length, self.log_n
+        n = 1 << log_n
+        generator, omega = stark.generator.value, stark.omega.value
+        if proof_stream is None:
+            proof_stream = sa_host.ip.ProofStream()
+        assert len(trace) == self.ncycles, \
+            "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
+
+        # trace randomizers (fast_stark.py:82-83), in the reference's order; the caller's list is not touched
+        rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
+                              for k in range(stark.num_randomizers)]
+
+        # trace polynomials (:86-90): one upload, one batched interpolation
+        columns = eng.upload(sa_devlist.pack([rows[c][s] for s in range(nregs) for c in range(T)]))
+        polys = eng.interp_apply(self.interp, columns.reshape(nregs, T, 2))
+
+        # boundary quotients (:93-106) into the first nregs rows of the commitment buffer
+        bplan = eng.boundary_plan(boundary, nregs, stark.omicron, log_n, omega, generator)
+        bounds_b = bplan.degree_bounds(T)
+        committed = eng.empty((nregs + 1) * n).reshape(nregs + 1, n, 2)
+        bquot, _, _ = eng.boundary_quotients(bplan, polys, check=True, out=committed[:nregs])
+
+        # transition quotients (:108-113), each constraint at the order the reference divides it at
+        tops = [_value(lo, hi) for lo, hi in eng.gather_batch(polys, [T - 1]).reshape(nregs, 2).tolist()]
+        quots = [eng.air_quotients(plan, polys, qlen) for _, plan, _, qlen in self.groups]
+        where = {}
+        for g, (_, _, idx, _) in enumerate(self.groups):
+            for j, c in enumerate(idx):
+                where[c] = (g, j)
+        long_rows = {}
+        for k in self.cons:
+            # a non-zero top coefficient makes the numerator's degree k.degree, so the reference's order is k.order
+            assert self._top_coefficient(k, tops), "sa_stark: the numerator of transition constraint %d is below " \
+                "its degree bound %d; its division order cannot be decided exactly" % (k.index, k.degree)
+            assert k.kind != "larger", LARGER_DEGREE
+            if k.kind == "long":
+                g, j = where[k.index]
+                if g not in long_rows:
+                    long_rows[g] = sa_marshal.unpack(eng.download(quots[g].reshape(-1, 2)), field, FieldElement)
+                qlen = self.groups[g][3]
+                tail = long_rows[g][j * qlen + k.bound + 1:(j + 1) * qlen]
+                assert not any(v.value for v in tail), REMAINDER
+
+        # randomizer polynomial (:116-119), drawn where the reference draws it, committed with the boundary codewords
+        randomizer = [field.sample(os.urandom(17)) for i in range(self.max_degree + 1)]
+        rvec = eng.upload(sa_devlist.pack(randomizer))
+        eng.coset_evaluate(rvec, log_n, omega, generator, out=committed[nregs])
+        trees = eng.merkle_trees(committed)
+        roots = eng.tree_roots(trees)
+        for root in roots:
+            proof_stream.push(root)
+
+        # weights (:125), then the degree check (:127): each quotient's coefficient at its bound is non-zero
+        weights = [w.value for w in stark.sample_weights(1 + 2 * len(self.cons) + 2 * nregs,
+                                                         proof_stream.prover_fiat_shamir())]
+        for g, (_, _, idx, qlen) in enumerate(self.groups):
+            if self.cons[idx[0]].kind == "transform":
+                at = [j * qlen + self.cons[c].bound for j, c in enumerate(idx)]
+                vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
+                assert all(int(lo) or int(hi) for lo, hi in vals), DEGREE_MISMATCH
+
+        # the combination (:129-148): each quotient truncated to its bound, at shift 0 and at max_degree - bound
+        terms = [(rvec, 0, weights[0])]
+        for k in self.cons:
+            g, j = where[k.index]
+            q = quots[g][j, :k.bound + 1]
+            terms += [(q, 0, weights[1 + 2 * k.index]), (q, self.max_degree - k.bound, weights[2 + 2 * k.index])]
+        base = 1 + 2 * len(self.cons)
+        for s, bound in enumerate(bounds_b):
+            q = bquot[s, :bound + 1]
+            terms += [(q, 0, weights[base + 2 * s]), (q, self.max_degree - bound, weights[base + 2 * s + 1])]
+        combined = eng.coset_combine_evaluate(terms, log_n, omega, generator)
+
+        # FRI (:151) on the device codeword
+        indices = self.fri.prove(sa_devlist.DeviceCodeword(combined, None, field, n), proof_stream)
+
+        # openings (:154-175)
+        duplicated = list(indices) + [(i + stark.expansion_factor) % n for i in indices]
+        quadrupled = duplicated + [(i + n // 2) % n for i in duplicated]
+        quadrupled.sort()
+        distinct = sorted(set(quadrupled))
+        raw = eng.gather_batch(committed, distinct)
+        paths = eng.merkle_open_batch(trees, quadrupled)
+        for b in range(nregs + 1):
+            # a repeated index pushes the same element object, as indexing one list does; every path is its own
+            values = dict(zip(distinct, sa_marshal.unpack(raw[b], field, FieldElement)))
+            for q, i in enumerate(quadrupled):
+                proof_stream.push(values[i])
+                proof_stream.push(paths[b][q])
+        zc = transition_zerofier_codeword
+        if isinstance(zc, sa_devlist.DeviceCodeword):
+            zc.prefetch(quadrupled)
+            zpaths = zc.open_paths(quadrupled)
+        else:
+            tree = _fri.Merkle._device_tree(zc)
+            zpaths = ([_fri.Merkle.open(i, zc) for i in quadrupled] if tree is None or len(zc) < 2
+                      else eng.merkle_open(tree, quadrupled))
+        for q, i in enumerate(quadrupled):
+            proof_stream.push(zc[i])
+            proof_stream.push(zpaths[q])
+        return proof_stream.serialize()
+
+
+def prove(stark, trace, transition_constraints, boundary, transition_zerofier, transition_zerofier_codeword,
+          proof_stream=None):
+    """FastStark.prove's signature and result through a StarkPlan built for this one call (no plan is cached)"""
+    plan = StarkPlan(stark, transition_constraints, transition_zerofier)
+    return plan.prove(trace, boundary, transition_zerofier_codeword, proof_stream)
+
+
+_originals = {}  # class -> its own `prove` attribute before enable (None: inherited)
+
+
+def enable(cls):
+    """rebind cls.prove (FastStark's, or a subclass's) to sa_stark.prove (idempotent)"""
+    if cls not in _originals:
+        _originals[cls] = cls.__dict__.get("prove")
+        cls.prove = prove
+
+
+def disable():
+    """restore every class enable rebound"""
+    for cls, orig in _originals.items():
+        if orig is None:
+            del cls.prove
+        else:
+            cls.prove = orig
+    _originals.clear()
