@@ -275,6 +275,22 @@ int sa_air_plan(void *plan, const uint64_t *coeffs, const uint32_t *exps, const 
  * conditions as sa_coset_div_apply_batch).  Reads the plan only: one plan may be applied on several streams at once. */
 int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
                      size_t ncons, int log_n, const uint64_t root[2], void *stream);
+/* code/stark.py:111: the same rows with an exact-division check.  out is exactly sa_air_quotients'; flags[c] = 0
+ * exactly when U_c[j] = 0 for every tail <= j < n (U_c above, the row before the offset^-j store).  With
+ * tail = n - deg Z it is the reference's remainder test of Polynomial.__truediv__ (univariate.py:50-53) for every
+ * numerator, N_c = 0 and deg N_c < deg Z included:
+ *   - the build guarantees deg N_c < n;
+ *   - if U_c vanishes from n - deg Z on, U_c * Z has degree below n and agrees with N_c on the n points x_i, so Z
+ *     divides N_c (and U_c is the quotient);
+ *   - conversely an exact quotient has degree deg N_c - deg Z < n - deg Z.
+ * SA_ESIZE before any launch for tail > n and for everything sa_air_quotients refuses; an error leaves out and flags
+ * untouched.  Launches: sa_air_quotients' plus one memset that clears the flags (the store is a warp ballot over the
+ * tail with one atomicOr per flagged row a warp touches, in place of the plain store).  Asynchronous: no host
+ * synchronisation, and no allocation once the stream's workspaces have grown, so the call can be captured in a CUDA
+ * graph; a replay clears the flags again.  Reads the plan only.                                                    */
+int sa_air_quotients_exact(void *out, uint32_t *flags, const void *plan, const void *trace, size_t nregs,
+                           size_t ncoef, size_t qlen, size_t ncons, size_t tail, int log_n, const uint64_t root[2],
+                           void *stream);
 
 /* ---- code/fast_stark.py:92-106: the boundary quotients, their coset codewords and a remainder check ------------
  * Register s has the trace polynomial T_s, the interpolant I_s of its boundary values and the zerofier Z_s of its

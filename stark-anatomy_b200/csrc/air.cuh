@@ -12,14 +12,22 @@
 // build checks it) N_c has degree < n, so its values determine it and the rows are fast_coset_divide's at order n,
 // bit for bit, clean division or not.
 //
+// The exact apply adds a remainder check: flags[c] = 0 exactly when U_c[j] = 0 for every tail <= j < n.  With
+// tail = n - deg Z that is the reference's test of N_c / Z (univariate.py:50-53) for every numerator, N_c = 0 and
+// deg N_c < deg Z included: the build keeps deg N_c < n, so if U_c vanishes from n - deg Z on, U_c Z has degree below
+// n and agrees with N_c on the n points x_i, hence Z divides N_c; conversely an exact quotient has degree
+// deg N_c - deg Z < n - deg Z, and N_c / Z = U_c on the coset.
+//
 // The schedules take the backend of coset.cuh plus b.pow_table_lead(out, base_m, lead_m, count) (k_pow_table with a
-// lead), b.upload(dst, host_src, count) and b.air_eval (k_air_eval).
+// lead), b.upload(dst, host_src, count) and b.air_eval (k_air_eval); the exact apply also b.clear_flags(flags, count)
+// (a memset in stream order) and b.air_store_exact (k_air_store_exact).
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <numeric>
 #include <vector>
 
+#include "boundary.cuh"  // boundary_flag_leader, shared by the exact store
 #include "coset.cuh"
 
 namespace sa {
@@ -87,6 +95,20 @@ SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, c
         }
     }
     for (; cur < c0 + nb; cur++, acc = fe_zero()) tile_st(V + (cur - c0) * n + i, fe_montmul(acc, iz));
+}
+
+// ---- element function: the body of k_air_store_exact ----
+// coset_store_elem's store of row b = idx >> log_n (out[b][j] = U[b][j] * offset^-j for j < qlen, U = ws) and whether
+// U[b][j] is a non-zero coefficient at j >= tail, i.e. part of a remainder; the rows are coset_store_elem's bit for
+// bit.  Indices from batch * n on, up to the warp's end, store nothing and return false: the kernel's ballot then
+// raises each row's flag once per warp with boundary_flag_leader.
+SA_HD bool air_store_exact_elem(fe *out, const fe *ws, const fe *ipw_m, long long qlen, long long tail, int log_n,
+                                long long batch, long long idx) {
+    if (idx >= batch << log_n) return false;
+    const long long b = idx >> log_n, j = idx & ((1ll << log_n) - 1);
+    const fe u = tile_ld(ws + idx);
+    if (j < qlen) tile_st(out + b * qlen + j, fe_montmul(u, tile_ld(ipw_m + j)));
+    return j >= tail && !fe_is_zero(u);
 }
 
 // ---- plan layout ----
@@ -157,6 +179,12 @@ inline int air_apply_check(int log_n, size_t nregs, size_t ncoef, size_t qlen, s
     if (nregs == 0 || ncons == 0) return SA_ESIZE;
     return coset_check(log_n, ncoef, qlen, root);
 }
+// the exact apply's: the apply's, and tail 0..n
+inline int air_exact_check(int log_n, size_t nregs, size_t ncoef, size_t qlen, size_t ncons, size_t tail,
+                           const uint64_t root[2]) {
+    SA_TRY(air_apply_check(log_n, nregs, ncoef, qlen, ncons, root));
+    return tail > ((size_t)1 << log_n) ? SA_ESIZE : SA_OK;
+}
 
 // ---- compilation (host) ----
 // the program of the terms term_start[0] .. term_start[ncons): the terms of each constraint sorted by (trace
@@ -209,12 +237,12 @@ int air_plan_build(B &b, fe *plan, const std::vector<fe> &prog, const fe *zerofi
 
 // The quotients of the plan's constraints for trace[nregs][ncoef] (coefficient rows): out[ncons][qlen].  The current
 // rows loaded with offset^i and the next rows with (offset * step)^j, one batched forward transform of the 2 nregs
-// rows, then per chunk of coset_batch_max(log_n) constraints k_air_eval, one batched inverse transform and the coset
-// store: 3 + 3 ceil(ncons / chunk) launches plus the transforms', whatever nregs and the chunk's size.
-// ws = air_ws_elems(nregs, ncons, log_n) elements.
-template <class B>
-int air_quotients(B &b, fe *out, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t qlen,
-                  size_t ncons, int log_n, const uint64_t root[2], fe *ws) {
+// rows, then per chunk of coset_batch_max(log_n) constraints k_air_eval, one batched inverse transform and
+// store(c0, nb, V), the chunk's store from V: 3 + 3 ceil(ncons / chunk) launches plus the transforms', whatever nregs
+// and the chunk's size.  ws = air_ws_elems(nregs, ncons, log_n) elements.
+template <class B, class Store>
+int air_apply(B &b, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t ncons, int log_n,
+              const uint64_t root[2], fe *ws, Store store) {
     const AirPlan L = air_plan_layout(log_n, 1, nregs, 0);
     const long long n = L.n;
     fe *ext = ws, *V = ws + 2 * nregs * (size_t)n;
@@ -227,9 +255,29 @@ int air_quotients(B &b, fe *out, const fe *plan, const fe *trace, size_t nregs, 
         SA_TRY(b.air_eval(V, plan + L.prog, plan + L.x, plan + L.div.inv, ext, (long long)c0, (long long)nb,
                           (int)nregs, log_n));
         SA_TRY(b.ntt(V, V, log_n, root, 1, nb));
-        SA_TRY(b.coset_store(out + c0 * qlen, V, plan + L.div.ipw, (long long)qlen, log_n, (long long)nb));
+        SA_TRY(store(c0, nb, V));
     }
     return SA_OK;
+}
+// the apply: k_coset_store per chunk
+template <class B>
+int air_quotients(B &b, fe *out, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t qlen,
+                  size_t ncons, int log_n, const uint64_t root[2], fe *ws) {
+    const fe *ipw = plan + air_plan_layout(log_n, 1, nregs, 0).div.ipw;
+    return air_apply(b, plan, trace, nregs, ncoef, ncons, log_n, root, ws, [&](size_t c0, size_t nb, const fe *V) {
+        return b.coset_store(out + c0 * qlen, V, ipw, (long long)qlen, log_n, (long long)nb);
+    });
+}
+// the exact apply: the flags[ncons] cleared first, then k_air_store_exact per chunk -- the apply's launches plus one
+template <class B>
+int air_quotients_exact(B &b, fe *out, uint32_t *flags, const fe *plan, const fe *trace, size_t nregs, size_t ncoef,
+                        size_t qlen, size_t ncons, size_t tail, int log_n, const uint64_t root[2], fe *ws) {
+    const fe *ipw = plan + air_plan_layout(log_n, 1, nregs, 0).div.ipw;
+    SA_TRY(b.clear_flags(flags, ncons));
+    return air_apply(b, plan, trace, nregs, ncoef, ncons, log_n, root, ws, [&](size_t c0, size_t nb, const fe *V) {
+        return b.air_store_exact(out + c0 * qlen, flags + c0, V, ipw, (long long)qlen, (long long)tail, log_n,
+                                 (long long)nb);
+    });
 }
 
 }  // namespace sa

@@ -237,6 +237,16 @@ __global__ void k_boundary_store(fe *quot, uint32_t *flags, const fe *ws, const 
         if (bad && boundary_flag_leader(ballot, threadIdx.x & 31, log_n)) atomicOr(flags + (idx >> log_n), 1u);
     });
 }
+// the exact apply's store: k_coset_store's rows and their remainder flags, with k_boundary_store's warp ballot (the
+// range rounded up to whole warps) and one atomicOr per row a warp touches at most
+__global__ void k_air_store_exact(fe *out, uint32_t *flags, const fe *ws, const fe *ipw_m, long long qlen,
+                                  long long tail, int log_n, long long batch) {
+    grid_stride(((batch << log_n) + 31) & ~31ll, [&](long long idx) {
+        const bool bad = air_store_exact_elem(out, ws, ipw_m, qlen, tail, log_n, batch, idx);
+        const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, bad);
+        if (bad && boundary_flag_leader(ballot, threadIdx.x & 31, log_n)) atomicOr(flags + (idx >> log_n), 1u);
+    });
+}
 
 extern "C" {
 
@@ -361,6 +371,12 @@ struct DeviceBoundary : DeviceAir {
     }
     int boundary_store(fe *q, uint32_t *flags, const fe *ws, const fe *ipw, const fe *deg, ll nc, int lg, ll nb) {
         return go(k_boundary_store, tree_grid(nb << lg), q, flags, ws, ipw, deg, nc, lg, nb);
+    }
+};
+// DeviceBoundary (its flags' memset) plus the store of the AIR's exact apply (air.cuh)
+struct DeviceAirExact : DeviceBoundary {
+    int air_store_exact(fe *o, uint32_t *flags, const fe *ws, const fe *ipw, ll q, ll tail, int lg, ll nb) {
+        return go(k_air_store_exact, tree_grid(nb << lg), o, flags, ws, ipw, q, tail, lg, nb);
     }
 };
 static int tree_workspace(Tree &t, cudaStream_t st) {
@@ -606,6 +622,19 @@ int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nreg
     SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, ncons, log_n), st, WS_AIR));
     DeviceAir b{{st}};
     return air_quotients(b, (fe *)out, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons, log_n, root, ws);
+}
+
+// sa_air_quotients plus the flags: the same workspace, one memset and the exact store in place of k_coset_store
+int sa_air_quotients_exact(void *out, uint32_t *flags, const void *plan, const void *trace, size_t nregs,
+                           size_t ncoef, size_t qlen, size_t ncons, size_t tail, int log_n, const uint64_t root[2],
+                           void *stream) {
+    SA_TRY(air_exact_check(log_n, nregs, ncoef, qlen, ncons, tail, root));
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, ncons, log_n), st, WS_AIR));
+    DeviceAirExact b{{{{st}}}};
+    return air_quotients_exact(b, (fe *)out, flags, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons,
+                               tail, log_n, root, ws);
 }
 
 // ---- boundary quotients (boundary.cuh) ----

@@ -70,6 +70,8 @@ SYMBOLS = [
     ("sa_air_plan", _ci, [_vp, _u64p, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(_sz), _sz, _sz, _sz, _vp, _sz,
                           _ci, _u64p, _u64p, _u64p, _vp]),
     ("sa_air_quotients", _ci, [_vp, _vp, _vp, _sz, _sz, _sz, _sz, _ci, _u64p, _vp]),
+    ("sa_air_quotients_exact", _ci, [_vp, ctypes.POINTER(ctypes.c_uint32), _vp, _vp, _sz, _sz, _sz, _sz, _sz, _ci,
+                                     _u64p, _vp]),
     ("sa_boundary_plan_bytes", _sz, [_ci, _sz]),
     ("sa_boundary_plan", _ci, [_vp, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_sz),
                                ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_sz), _sz, _ci, _u64p, _u64p, _vp]),
@@ -138,10 +140,11 @@ class CosetDivPlan:
 
 class AirPlan:
     """A transition quotient plan (CudaEngine.air_plan): the device buffer sa_air_plan filled (torch.uint8) for one
-    AIR and zerofier on the coset offset * <root> of order 2^log_n, with the values every apply passes again"""
-    __slots__ = ("plan", "log_n", "root", "offset", "nregs", "ncons", "max_ncoef")
+    AIR and zerofier on the coset offset * <root> of order 2^log_n, with the values every apply passes again and the
+    zerofier's degree (its length - 1; None where unknown), which the exact apply's tail needs"""
+    __slots__ = ("plan", "log_n", "root", "offset", "nregs", "ncons", "max_ncoef", "zdeg")
 
-    def __init__(self, plan, log_n, root, offset, nregs, ncons, max_ncoef):
+    def __init__(self, plan, log_n, root, offset, nregs, ncons, max_ncoef, zdeg=None):
         self.plan = plan
         self.log_n = log_n
         self.root = root
@@ -149,6 +152,7 @@ class AirPlan:
         self.nregs = nregs
         self.ncons = ncons
         self.max_ncoef = max_ncoef
+        self.zdeg = zdeg
 
 
 class BoundaryPlan:
@@ -491,7 +495,7 @@ class CudaEngine:
             (ctypes.c_uint32 * max(len(exps), 1))(*exps), (ctypes.c_size_t * (ncons + 1))(*starts), ncons, nregs,
             max_ncoef, zerofier.data_ptr(), zerofier.shape[0], log_n, _limbs(root), _limbs(offset), _limbs(step),
             self._stream()))
-        return AirPlan(plan, log_n, int(root), int(offset), nregs, ncons, max_ncoef)
+        return AirPlan(plan, log_n, int(root), int(offset), nregs, ncons, max_ncoef, zerofier.shape[0] - 1)
 
     def air_quotients(self, plan, trace, qlen):
         """sa_air_quotients: the first qlen coefficients of every constraint's quotient for the trace polynomials
@@ -509,6 +513,32 @@ class CudaEngine:
                                               trace.shape[1], int(qlen), plan.ncons, plan.log_n, _limbs(plan.root),
                                               self._stream()))
         return out
+
+    def air_quotients_exact(self, plan, trace, qlen, check=True):
+        """sa_air_quotients_exact: air_quotients' rows (ncons, qlen, 2) and the remainder flags (ncons,) int32,
+        non-zero exactly where Z does not divide the constraint's numerator (the reference's Polynomial.__truediv__
+        test), with the tail n - deg Z.  The zerofier's top coefficient must be non-zero (deg Z = its length - 1, as
+        air_plan takes it).  check=True reads the flags (one synchronisation) and raises the reference's remainder
+        message naming the constraints; check=False stays asynchronous.  The plan is only read."""
+        torch = self.torch
+        if (not isinstance(trace, torch.Tensor) or trace.dtype != torch.int64 or trace.device != self.device
+                or trace.dim() != 3 or trace.shape[0] != plan.nregs or trace.shape[2] != 2
+                or not 1 <= trace.shape[1] <= plan.max_ncoef or not 1 <= int(qlen) <= 1 << plan.log_n
+                or plan.zdeg is None):
+            raise SaError(SA_ERRORS[-6])
+        trace = trace.contiguous()
+        out = torch.empty((plan.ncons, int(qlen), 2), dtype=torch.int64, device=self.device)
+        flags = torch.empty(plan.ncons, dtype=torch.int32, device=self.device)
+        self._check(self.lib.sa_air_quotients_exact(
+            out.data_ptr(), ctypes.cast(flags.data_ptr(), ctypes.POINTER(ctypes.c_uint32)), plan.plan.data_ptr(),
+            trace.data_ptr(), plan.nregs, trace.shape[1], int(qlen), plan.ncons, (1 << plan.log_n) - plan.zdeg,
+            plan.log_n, _limbs(plan.root), self._stream()))
+        if check:
+            self._count("d2h", 4 * plan.ncons)
+            bad = [c for c, f in enumerate(flags.tolist()) if f]
+            if bad:
+                raise SaError("%s (constraints %s)" % (REMAINDER, bad))
+        return out, flags
 
     def _ints(self, values):
         """a list of ints -> device vector (n, 2)"""

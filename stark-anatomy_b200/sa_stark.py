@@ -1,4 +1,5 @@
-"""sa_stark -- FastStark.prove on the device: from the trace to the serialized proof through the planned stages.
+"""sa_stark -- FastStark.prove and Stark.prove on the device: from the trace to the serialized proof through the
+planned stages.
 
 The reference's prover (code/fast_stark.py:76-178) interpolates the trace, divides out the boundary and the
 transition zerofiers, commits, combines and runs FRI in Python.  ``StarkPlan.prove`` runs the same schedule through
@@ -21,8 +22,14 @@ the engine's planned calls, and only roots, challenges and opened leaves cross t
 The proof bytes are the reference's (DESIGN section 3.9 gives the argument), or an AssertionError: inputs this
 schedule cannot decide exactly are refused rather than proven differently.
 
-``enable(cls)`` rebinds ``cls.prove`` (FastStark's) to ``prove``; ``disable()`` restores it.  Off by default, as
-``sa_accel``.  Nothing here imports torch or holds device state outside a ``StarkPlan``.
+``PlainStarkPlan.prove`` is the same schedule for stark.py's plain prover (Stark.prove, stark.py:73-170, and so
+RPSSS.sign): the stages above are shared code, the transition quotients come from ``air_quotients_exact``, whose
+per-constraint flag is exactly the reference's exact-division test (DESIGN section 3.10), and there are no zerofier
+openings.
+
+``enable(cls)`` rebinds ``cls.prove`` (FastStark's) to ``prove``, ``enable_plain(cls)`` rebinds Stark's to
+``prove_plain``; ``disable()`` restores both.  Off by default, as ``sa_accel``.  Nothing here imports torch or holds
+device state outside a plan.
 """
 import os
 from hashlib import blake2b
@@ -129,7 +136,95 @@ class _Constraint:
     __slots__ = ("index", "degree", "bound", "top", "kind", "order")
 
 
-class StarkPlan:
+class _Stages:
+    """The stages FastStark's and Stark's provers share (fast_stark.py:82-106, 116-125, 129-169; stark.py:79-104,
+    113-123, 127-167): the trace randomizers and one batched interpolation, the boundary quotients into the first
+    nregs rows of the commitment buffer, the randomizer polynomial next to them and one commitment of all nregs + 1
+    codewords, the weights, the combination, FRI on the device codeword and the openings of the committed codewords.
+    A plan sets stark, fri, nregs, ncycles, trace_length, log_n, max_degree and interp."""
+
+    def _setup(self, stark, n):
+        """fri (the drop-in Fri of the FRI domain of n points) and interp (the randomized trace domain's plan)"""
+        eng = sa_engine.get_engine()
+        fri = getattr(stark, "fri", None)
+        self.fri = fri if isinstance(fri, _fri.Fri) else _fri.Fri(
+            stark.generator, stark.omega, n, stark.expansion_factor, stark.num_colinearity_checks)
+        omicron = stark.omicron.value
+        domain = [FieldElement(pow(omicron, i, P), stark.field) for i in range(self.trace_length)]
+        self.interp = eng.interp_plan(eng.upload(sa_devlist.pack(domain)))
+
+    def _trace_polynomials(self, eng, trace):
+        """the trace randomizers, drawn in the reference's order (the caller's list is not touched), one upload of
+        the columns and one batched interpolation: the (nregs, T, 2) trace polynomials"""
+        stark, field, nregs, T = self.stark, self.stark.field, self.nregs, self.trace_length
+        assert len(trace) == self.ncycles, \
+            "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
+        rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
+                              for k in range(stark.num_randomizers)]
+        columns = eng.upload(sa_devlist.pack([rows[c][s] for s in range(nregs) for c in range(T)]))
+        return eng.interp_apply(self.interp, columns.reshape(nregs, T, 2))
+
+    def _boundary(self, eng, polys, boundary):
+        """(the (nregs + 1, n, 2) commitment buffer with the boundary codewords in its first rows, the boundary
+        quotients, their degree bounds); the reference's remainder message when a boundary value is false"""
+        stark, nregs, log_n = self.stark, self.nregs, self.log_n
+        bplan = eng.boundary_plan(boundary, nregs, stark.omicron, log_n, stark.omega.value, stark.generator.value)
+        committed = eng.empty((nregs + 1) << log_n).reshape(nregs + 1, 1 << log_n, 2)
+        bquot, _, _ = eng.boundary_quotients(bplan, polys, check=True, out=committed[:nregs])
+        return committed, bquot, bplan.degree_bounds(self.trace_length)
+
+    def _commit(self, eng, committed, proof_stream):
+        """the randomizer polynomial, drawn where the reference draws it, its codeword in the buffer's last row, one
+        commitment of every row and their roots pushed in order: (the randomizer, the trees)"""
+        stark, nregs, log_n = self.stark, self.nregs, self.log_n
+        randomizer = [stark.field.sample(os.urandom(17)) for i in range(self.max_degree + 1)]
+        rvec = eng.upload(sa_devlist.pack(randomizer))
+        eng.coset_evaluate(rvec, log_n, stark.omega.value, stark.generator.value, out=committed[nregs])
+        trees = eng.merkle_trees(committed)
+        for root in eng.tree_roots(trees):
+            proof_stream.push(root)
+        return rvec, trees
+
+    def _weights(self, proof_stream):
+        """1 + 2 ncons + 2 nregs weights from the caller's prover_fiat_shamir()"""
+        number = 1 + 2 * len(self.constraints) + 2 * self.nregs
+        return [w.value for w in self.stark.sample_weights(number, proof_stream.prover_fiat_shamir())]
+
+    def _combine_prove_open(self, eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_stream):
+        """the combination of the randomizer, each transition quotient row (rows: (the row truncated to its bound
+        + 1, the bound)) and each boundary quotient at shift 0 and at max_degree - bound; FRI on its codeword; the
+        openings of the committed codewords.  An empty row (a zero quotient) adds nothing and is left out.
+        Returns the quadrupled indices."""
+        stark, field, nregs, log_n = self.stark, self.stark.field, self.nregs, self.log_n
+        n = 1 << log_n
+        terms = [(rvec, 0, weights[0])]
+        for c, (q, bound) in enumerate(rows):
+            if bound >= 0:
+                terms += [(q, 0, weights[1 + 2 * c]), (q, self.max_degree - bound, weights[2 + 2 * c])]
+        base = 1 + 2 * len(rows)
+        for s, bound in enumerate(bounds_b):
+            q = bquot[s, :bound + 1]
+            terms += [(q, 0, weights[base + 2 * s]), (q, self.max_degree - bound, weights[base + 2 * s + 1])]
+        combined = eng.coset_combine_evaluate(terms, log_n, stark.omega.value, stark.generator.value)
+
+        indices = self.fri.prove(sa_devlist.DeviceCodeword(combined, None, field, n), proof_stream)
+
+        duplicated = list(indices) + [(i + stark.expansion_factor) % n for i in indices]
+        quadrupled = duplicated + [(i + n // 2) % n for i in duplicated]
+        quadrupled.sort()
+        distinct = sorted(set(quadrupled))
+        raw = eng.gather_batch(committed, distinct)
+        paths = eng.merkle_open_batch(trees, quadrupled)
+        for b in range(nregs + 1):
+            # a repeated index pushes the same element object, as indexing one list does; every path is its own
+            values = dict(zip(distinct, sa_marshal.unpack(raw[b], field, FieldElement)))
+            for q, i in enumerate(quadrupled):
+                proof_stream.push(values[i])
+                proof_stream.push(paths[b][q])
+        return quadrupled
+
+
+class StarkPlan(_Stages):
     """What does not change between proofs of one AIR on one FastStark (or ``Params``): the interpolation plan of
     the randomized trace domain, one AIR plan per division order with the zerofier uploaded once, and the
     constraints' degrees, bounds and shifts.  Only read by ``prove``."""
@@ -146,10 +241,7 @@ class StarkPlan:
         self.log_n = n.bit_length() - 1
         omicron = stark.omicron.value
         T = self.trace_length
-
-        fri = getattr(stark, "fri", None)
-        self.fri = fri if isinstance(fri, _fri.Fri) else _fri.Fri(
-            stark.generator, stark.omega, n, stark.expansion_factor, stark.num_colinearity_checks)
+        self._setup(stark, n)
 
         zerofier = _ints(getattr(transition_zerofier, "coefficients", transition_zerofier))
         zdeg = _degree(zerofier)
@@ -200,8 +292,9 @@ class StarkPlan:
                                 pow(omicron, odl // order, P), stark.generator.value, omicron)
             self.groups.append((order, plan, idx, order if long else max(self.cons[c].bound for c in idx) + 1))
 
-        domain = [FieldElement(pow(omicron, i, P), field) for i in range(T)]
-        self.interp = eng.interp_plan(eng.upload(sa_devlist.pack(domain)))
+    def _where(self):
+        """constraint index -> (its group, its row in the group)"""
+        return {c: (g, j) for g, (_, _, idx, _) in enumerate(self.groups) for j, c in enumerate(idx)}
 
     def _top_coefficient(self, k, tops):
         """the coefficient of x^degree in constraint k's numerator: its maximal-degree terms on the trace
@@ -222,37 +315,18 @@ class StarkPlan:
         """FastStark.prove(trace, constraints, boundary, zerofier, zerofier_codeword, proof_stream) for this plan's
         constraints and zerofier: proof_stream.serialize()"""
         eng = sa_engine.get_engine()
-        stark = self.stark
-        field = stark.field
-        nregs, T, log_n = self.nregs, self.trace_length, self.log_n
-        n = 1 << log_n
-        generator, omega = stark.generator.value, stark.omega.value
+        T = self.trace_length
         if proof_stream is None:
             proof_stream = sa_host.ip.ProofStream()
-        assert len(trace) == self.ncycles, \
-            "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
 
-        # trace randomizers (fast_stark.py:82-83), in the reference's order; the caller's list is not touched
-        rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
-                              for k in range(stark.num_randomizers)]
-
-        # trace polynomials (:86-90): one upload, one batched interpolation
-        columns = eng.upload(sa_devlist.pack([rows[c][s] for s in range(nregs) for c in range(T)]))
-        polys = eng.interp_apply(self.interp, columns.reshape(nregs, T, 2))
-
-        # boundary quotients (:93-106) into the first nregs rows of the commitment buffer
-        bplan = eng.boundary_plan(boundary, nregs, stark.omicron, log_n, omega, generator)
-        bounds_b = bplan.degree_bounds(T)
-        committed = eng.empty((nregs + 1) * n).reshape(nregs + 1, n, 2)
-        bquot, _, _ = eng.boundary_quotients(bplan, polys, check=True, out=committed[:nregs])
+        # trace randomizers and trace polynomials (:82-90), boundary quotients (:93-106)
+        polys = self._trace_polynomials(eng, trace)
+        committed, bquot, bounds_b = self._boundary(eng, polys, boundary)
 
         # transition quotients (:108-113), each constraint at the order the reference divides it at
-        tops = [_value(lo, hi) for lo, hi in eng.gather_batch(polys, [T - 1]).reshape(nregs, 2).tolist()]
+        tops = [_value(lo, hi) for lo, hi in eng.gather_batch(polys, [T - 1]).reshape(self.nregs, 2).tolist()]
         quots = [eng.air_quotients(plan, polys, qlen) for _, plan, _, qlen in self.groups]
-        where = {}
-        for g, (_, _, idx, _) in enumerate(self.groups):
-            for j, c in enumerate(idx):
-                where[c] = (g, j)
+        where = self._where()
         long_rows = {}
         for k in self.cons:
             # a non-zero top coefficient makes the numerator's degree k.degree, so the reference's order is k.order
@@ -262,57 +336,32 @@ class StarkPlan:
             if k.kind == "long":
                 g, j = where[k.index]
                 if g not in long_rows:
-                    long_rows[g] = sa_marshal.unpack(eng.download(quots[g].reshape(-1, 2)), field, FieldElement)
+                    long_rows[g] = sa_marshal.unpack(eng.download(quots[g].reshape(-1, 2)), self.stark.field,
+                                                     FieldElement)
                 qlen = self.groups[g][3]
                 tail = long_rows[g][j * qlen + k.bound + 1:(j + 1) * qlen]
                 assert not any(v.value for v in tail), REMAINDER
 
-        # randomizer polynomial (:116-119), drawn where the reference draws it, committed with the boundary codewords
-        randomizer = [field.sample(os.urandom(17)) for i in range(self.max_degree + 1)]
-        rvec = eng.upload(sa_devlist.pack(randomizer))
-        eng.coset_evaluate(rvec, log_n, omega, generator, out=committed[nregs])
-        trees = eng.merkle_trees(committed)
-        roots = eng.tree_roots(trees)
-        for root in roots:
-            proof_stream.push(root)
+        # randomizer polynomial and the commitment (:116-119), weights (:125)
+        rvec, trees = self._commit(eng, committed, proof_stream)
+        weights = self._weights(proof_stream)
 
-        # weights (:125), then the degree check (:127): each quotient's coefficient at its bound is non-zero
-        weights = [w.value for w in stark.sample_weights(1 + 2 * len(self.cons) + 2 * nregs,
-                                                         proof_stream.prover_fiat_shamir())]
+        # the degree check (:127): each quotient's coefficient at its bound is non-zero
         for g, (_, _, idx, qlen) in enumerate(self.groups):
             if self.cons[idx[0]].kind == "transform":
                 at = [j * qlen + self.cons[c].bound for j, c in enumerate(idx)]
                 vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
                 assert all(int(lo) or int(hi) for lo, hi in vals), DEGREE_MISMATCH
 
-        # the combination (:129-148): each quotient truncated to its bound, at shift 0 and at max_degree - bound
-        terms = [(rvec, 0, weights[0])]
+        # the combination (:129-148), FRI (:151) and the boundary and randomizer openings (:154-169)
+        rows = []
         for k in self.cons:
             g, j = where[k.index]
-            q = quots[g][j, :k.bound + 1]
-            terms += [(q, 0, weights[1 + 2 * k.index]), (q, self.max_degree - k.bound, weights[2 + 2 * k.index])]
-        base = 1 + 2 * len(self.cons)
-        for s, bound in enumerate(bounds_b):
-            q = bquot[s, :bound + 1]
-            terms += [(q, 0, weights[base + 2 * s]), (q, self.max_degree - bound, weights[base + 2 * s + 1])]
-        combined = eng.coset_combine_evaluate(terms, log_n, omega, generator)
+            rows.append((quots[g][j, :k.bound + 1], k.bound))
+        quadrupled = self._combine_prove_open(eng, rvec, rows, bquot, bounds_b, weights, committed, trees,
+                                              proof_stream)
 
-        # FRI (:151) on the device codeword
-        indices = self.fri.prove(sa_devlist.DeviceCodeword(combined, None, field, n), proof_stream)
-
-        # openings (:154-175)
-        duplicated = list(indices) + [(i + stark.expansion_factor) % n for i in indices]
-        quadrupled = duplicated + [(i + n // 2) % n for i in duplicated]
-        quadrupled.sort()
-        distinct = sorted(set(quadrupled))
-        raw = eng.gather_batch(committed, distinct)
-        paths = eng.merkle_open_batch(trees, quadrupled)
-        for b in range(nregs + 1):
-            # a repeated index pushes the same element object, as indexing one list does; every path is its own
-            values = dict(zip(distinct, sa_marshal.unpack(raw[b], field, FieldElement)))
-            for q, i in enumerate(quadrupled):
-                proof_stream.push(values[i])
-                proof_stream.push(paths[b][q])
+        # ... and the zerofier's (:171-175)
         zc = transition_zerofier_codeword
         if isinstance(zc, sa_devlist.DeviceCodeword):
             zc.prefetch(quadrupled)
@@ -334,6 +383,108 @@ def prove(stark, trace, transition_constraints, boundary, transition_zerofier, t
     return plan.prove(trace, boundary, transition_zerofier_codeword, proof_stream)
 
 
+class PlainStarkPlan(_Stages):
+    """What does not change between proofs of one AIR on one Stark (stark.py's plain prover): the interpolation plan
+    of the randomized trace domain, the transition zerofier built on the device over omicron^0 .. omicron^(ncycles -
+    2) (Stark has no preprocess), one AIR plan per division order, and the constraints' bounds.  Stark keeps neither
+    the omicron domain's nor the FRI domain's length as attributes: they come from len(stark.omicron_domain) and
+    stark.fri.domain_length.  Only read by ``prove``.
+
+    The reference divides each transition numerator by Polynomial.__truediv__, an exact division, so the division
+    order never changes its result: constraint c (numerator degree bound D_c, T the randomized trace length) divides
+    at 2^max(bits(D_c), bits(T - 1)) with an exact-division flag, and a flag raises the remainder message.  Refused
+    with an AssertionError rather than proven otherwise: a division order above 2^30, a combination of max_degree + 1
+    coefficients above the FRI domain (the reference evaluates it there, but it does not fold), and the boundary
+    lists the boundary plan refuses."""
+
+    def __init__(self, stark, transition_constraints):
+        eng = sa_engine.get_engine()
+        self.stark = stark
+        field = stark.field
+        nregs = stark.num_registers
+        self.nregs = nregs
+        self.ncycles = stark.original_trace_length
+        self.trace_length = T = self.ncycles + stark.num_randomizers
+        n = stark.fri.domain_length
+        self.log_n = n.bit_length() - 1
+        omicron = stark.omicron.value
+        self._setup(stark, n)
+
+        self.constraints = list(transition_constraints)
+        zdeg = self.ncycles - 1
+        self.bounds, orders = [], []
+        for c, a in enumerate(self.constraints):
+            terms = _terms(a)
+            if any(len(k) > 1 + 2 * nregs for k, _ in terms):
+                raise AssertionError(sa_engine.SA_ERRORS[-6])
+            degree = max(_term_degree(e, T - 1) for e, _ in terms)  # ValueError without terms, as the reference's
+            self.bounds.append(degree - zdeg)
+            order = 1 << max(_bits(degree), _bits(T - 1))
+            assert order <= 1 << 30, "sa_stark: transition constraint %d has degree %d; its division order %d is " \
+                "above 2^30" % (c, degree, order)
+            orders.append(order)
+        self.max_degree = (1 << _bits(max(self.bounds))) - 1
+        assert self.max_degree + 1 <= n, "sa_stark: the combination has max_degree + 1 = %d coefficients, above " \
+            "the FRI domain's %d" % (self.max_degree + 1, n)
+
+        # the zerofier of omicron^0 .. omicron^(ncycles - 2) on the device; none for one cycle, where the reference's
+        # transition_zerofier raises IndexError at the division (prove raises it there)
+        self.groups = []  # (AirPlan, constraint indices, qlen)
+        if self.ncycles < 2:
+            return
+        points = [FieldElement(pow(omicron, i, P), field) for i in range(self.ncycles - 1)]
+        self.zerofier = eng.zerofier(eng.upload(sa_devlist.pack(points)))
+        for order in sorted(set(orders)):
+            idx = [c for c, o in enumerate(orders) if o == order]
+            plan = eng.air_plan([self.constraints[c] for c in idx], nregs, self.zerofier, T, order.bit_length() - 1,
+                                field.primitive_nth_root(order).value, stark.generator.value, omicron)
+            self.groups.append((plan, idx, max(1, max(self.bounds[c] for c in idx) + 1)))
+
+    def prove(self, trace, boundary, proof_stream=None):
+        """Stark.prove(trace, constraints, boundary, proof_stream) for this plan's constraints:
+        proof_stream.serialize()"""
+        eng = sa_engine.get_engine()
+        if proof_stream is None:
+            proof_stream = sa_host.ip.ProofStream()
+
+        # trace randomizers and trace polynomials (stark.py:79-87), boundary quotients (:90-104)
+        polys = self._trace_polynomials(eng, trace)
+        committed, bquot, bounds_b = self._boundary(eng, polys, boundary)
+
+        # transition quotients (:107-111): exact divisions, the remainder message before the randomizer is drawn
+        if not self.groups:
+            raise IndexError("list index out of range")  # zerofier_domain of no points (univariate.py:123)
+        quots = [eng.air_quotients_exact(plan, polys, qlen, check=True)[0] for plan, _, qlen in self.groups]
+
+        # randomizer polynomial and the commitment (:114-117), weights (:123)
+        rvec, trees = self._commit(eng, committed, proof_stream)
+        weights = self._weights(proof_stream)
+
+        # the degree check (:125).  A clean row U_c vanishes above deg N_c - deg Z <= b_c, so the quotient has
+        # degree b_c exactly when U_c[b_c] != 0.  For b_c < 0, deg N_c <= D_c < deg Z and Z | N_c force N_c = 0: the
+        # quotient is Polynomial([]), of degree -1 (univariate.py:8-9, 83-84), which matches b_c = -1 only.
+        ok = all(b >= -1 for b in self.bounds)
+        for g, (_, idx, qlen) in enumerate(self.groups):
+            at = [j * qlen + self.bounds[c] for j, c in enumerate(idx) if self.bounds[c] >= 0]
+            if at:
+                vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
+                ok = ok and all(int(lo) or int(hi) for lo, hi in vals)
+        assert ok, DEGREE_MISMATCH
+
+        # the combination (:127-146), FRI (:149) and the boundary and randomizer openings (:152-167)
+        rows = [None] * len(self.constraints)
+        for g, (_, idx, _) in enumerate(self.groups):
+            for j, c in enumerate(idx):
+                rows[c] = (quots[g][j, :max(0, self.bounds[c] + 1)], self.bounds[c])
+        self._combine_prove_open(eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_stream)
+        return proof_stream.serialize()
+
+
+def prove_plain(stark, trace, transition_constraints, boundary, proof_stream=None):
+    """Stark.prove's signature and result through a PlainStarkPlan built for this one call (no plan is cached)"""
+    return PlainStarkPlan(stark, transition_constraints).prove(trace, boundary, proof_stream)
+
+
 _originals = {}  # class -> its own `prove` attribute before enable (None: inherited)
 
 
@@ -344,8 +495,16 @@ def enable(cls):
         cls.prove = prove
 
 
+def enable_plain(cls):
+    """rebind cls.prove (Stark's, or a subclass's) to sa_stark.prove_plain (idempotent), so that RPSSS.sign runs
+    unmodified"""
+    if cls not in _originals:
+        _originals[cls] = cls.__dict__.get("prove")
+        cls.prove = prove_plain
+
+
 def disable():
-    """restore every class enable rebound"""
+    """restore every class enable and enable_plain rebound"""
     for cls, orig in _originals.items():
         if orig is None:
             del cls.prove
