@@ -234,6 +234,19 @@ int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log
 int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
                               const void *const *srcs, const size_t *lens, const size_t *shifts,
                               const uint64_t *weights, size_t nterms, void *stream);
+/* Many combinations in one call: term t is added into destination row rows[t] < nrows (a HOST array like the others),
+ * and out[r*n .. r*n+n) is row r's combination evaluated as above -- the codeword sa_coset_combine_evaluate gives for
+ * the terms of row r alone, zeros for a row without terms.  Rows are contiguous; out must not overlap any source.
+ * Launches: one offset^i table of the longest row's ncomb elements, one per group of 64 terms over all rows, one
+ * batched forward sa_ntt of the nrows rows in place: 1 + ceil(nterms / 64) plus the batched transform's, whatever
+ * nrows -- no launch per row.  sa_coset_combine_evaluate is nrows = 1 of the same kernel.  Before any launch:
+ * sa_coset_combine_evaluate's checks and SA_ESIZE for any rows[t] >= nrows; an error leaves out untouched.
+ * nrows == 0 (and so no term) returns SA_OK without a launch.  The same asynchronous and graph-capture promises as
+ * sa_coset_combine_evaluate.                                                                                       */
+int sa_coset_combine_evaluate_batch(void *out, size_t nrows, int log_n, const uint64_t root[2],
+                                    const uint64_t offset[2], const void *const *srcs, const size_t *lens,
+                                    const size_t *shifts, const size_t *rows, const uint64_t *weights, size_t nterms,
+                                    void *stream);
 /* The most rows one chunk of sa_coset_div_apply_batch / sa_coset_evaluate_batch takes:
  * max(1, floor(2^30 / (32 n))) (32 at 2^20, 512 at 2^16), so a chunk's workspace stays at or below
  * 1 GiB; 0 when log_n is outside 1..30.  Host-only: no CUDA call.                                */
@@ -291,6 +304,26 @@ int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nreg
 int sa_air_quotients_exact(void *out, uint32_t *flags, const void *plan, const void *trace, size_t nregs,
                            size_t ncoef, size_t qlen, size_t ncons, size_t tail, int log_n, const uint64_t root[2],
                            void *stream);
+/* The same applies for `batch` traces of one AIR in one call: trace[batch][nregs][ncoef] gives out[batch][ncons][qlen]
+ * (and flags[batch][ncons]), trace b's rows (and flags) exactly what sa_air_quotients (sa_air_quotients_exact) gives
+ * for trace b alone.  sa_air_quotients and sa_air_quotients_exact are batch 1, with the launches they always had.
+ * The batch runs in chunks of whole traces, sa_air_batch_max(nregs, ncons, log_n) at most; a chunk issues the
+ * launches of one trace's apply (two coset loads of all its traces' rows, one batched forward sa_ntt, then the
+ * evaluation kernel, one batched inverse sa_ntt and the store per row chunk of at most sa_coset_batch_max(log_n)
+ * constraint rows; the exact apply's flags memset once per call).  Per-stream workspace: 16*n*(2*nregs*traces +
+ * rows) bytes for a chunk of `traces` traces and row chunks of `rows` rows, besides the transform's.  The same checks
+ * before any launch as the single calls (an error leaves out and flags untouched); batch == 0 returns SA_OK without a
+ * launch.  The same asynchronous and graph-capture promises; the plan is only read.                               */
+int sa_air_quotients_batch(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
+                           size_t ncons, size_t batch, int log_n, const uint64_t root[2], void *stream);
+int sa_air_quotients_exact_batch(void *out, uint32_t *flags, const void *plan, const void *trace, size_t nregs,
+                                 size_t ncoef, size_t qlen, size_t ncons, size_t batch, size_t tail, int log_n,
+                                 const uint64_t root[2], void *stream);
+/* The most traces one chunk of a batched apply takes: max(1, floor(sa_coset_batch_max(log_n) / (2*nregs + ncons))),
+ * so that a chunk of several traces keeps its 2*nregs transformed trace rows and ncons constraint rows per trace at
+ * 32*n bytes per row with the transform's -- at most 1 GiB per stream -- and is one row chunk (64 traces of 2
+ * registers and 4 constraints at 2^16, 4 at 2^20); 0 when log_n is outside 1..30.  Host-only: no CUDA call.        */
+size_t sa_air_batch_max(size_t nregs, size_t ncons, int log_n);
 
 /* ---- code/fast_stark.py:92-106: the boundary quotients, their coset codewords and a remainder check ------------
  * Register s has the trace polynomial T_s, the interpolant I_s of its boundary values and the zerofier Z_s of its
@@ -361,6 +394,18 @@ int sa_gather(void *out, const void *values, size_t n, const uint64_t *indices_h
  * Asynchronous.                                                                           */
 int sa_gather_batch(void *out, const void *values, size_t n, size_t batch, const uint64_t *indices_host, size_t k,
                     void *stream);
+/* Openings with an index set per group of rows: rows (trees) are taken in groups of `group`, and group g reads its
+ * own k indices from indices_host[g*k .. g*k+k), ceil(batch / group) sets (one when batch == 0).  So
+ * out[b*k + q] = values[b*n + indices_host[(b / group)*k + q]] and paths_out[b][q][level] is the sibling at `level`
+ * of leaf indices_host[(b / group)*k + q] in tree b.  With the committed rows of many proofs back to back, group =
+ * rows per proof opens every proof's rows at that proof's own indices in one call.  sa_gather_batch and
+ * sa_merkle_open_batch are group = batch of the same kernels.  Before any launch: SA_ESIZE for group == 0, and
+ * everything the ungrouped calls refuse (SA_EINDEX for any index of any set >= n).  One index upload, one launch;
+ * the same cases without a launch as the ungrouped calls.  Asynchronous.                                           */
+int sa_gather_batch_sets(void *out, const void *values, size_t n, size_t batch, size_t group,
+                         const uint64_t *indices_host, size_t k, void *stream);
+int sa_merkle_open_batch_sets(void *paths_out, const void *trees, size_t n, size_t batch, size_t group,
+                              const uint64_t *indices_host, size_t k, void *stream);
 
 /* ---- code/fri.py:85 split-and-fold, and the fused round of Fri.commit (fri.py:64-88) ----
  * next[i] = 2^-1 * ((1 + alpha/(offset*omega^i)) * cw[i] + (1 - alpha/(offset*omega^i)) * cw[n/2+i])

@@ -18,9 +18,13 @@
 // n and agrees with N_c on the n points x_i, hence Z divides N_c; conversely an exact quotient has degree
 // deg N_c - deg Z < n - deg Z, and N_c / Z = U_c on the coset.
 //
+// An apply takes a batch of traces, trace[batch][nregs][ncoef] -> out[batch][ncons][qlen]: row b * ncons + c is
+// constraint c of trace b, the row the apply of trace b alone gives.  A batch shares the launches of one apply within
+// a chunk (air_chunks below); the single-trace apply is batch 1.
+//
 // The schedules take the backend of coset.cuh plus b.pow_table_lead(out, base_m, lead_m, count) (k_pow_table with a
-// lead), b.upload(dst, host_src, count) and b.air_eval (k_air_eval); the exact apply also b.clear_flags(flags, count)
-// (a memset in stream order) and b.air_store_exact (k_air_store_exact).
+// lead), b.upload(dst, host_src, count) and b.air_eval (k_air_eval, air_eval_rows_elem); the exact apply also
+// b.clear_flags(flags, count) (a memset in stream order) and b.air_store_exact (k_air_store_exact).
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -56,17 +60,17 @@ SA_HD fe air_pow(const fe &b_m, uint32_t e) {
     return acc;
 }
 
-// ---- element function: the body of k_air_eval for one point ----
-// V[c - c0][i] = N_c(x_i) / Z(x_i) for the constraints c0 <= c < c0 + nb, walking the program once: records of other
-// constraints are skipped, a constraint without records gets zeros.  x_m and iz_m are the plan's x_i and 1/Z_i, ext
-// the 2 nregs rows T_s(x_i), T_s(step * x_i) (canonical); coefficients are canonical, so a coefficient times a
-// Montgomery-form power is canonical again  (i < n)
-SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long c0,
-                         long long nb, int nregs, int log_n, long long i) {
+// ---- element functions: the body of k_air_eval for one point ----
+// V[c - c0][i] = N_c(x_i) / Z(x_i) for the constraints c0 <= c < c0 + nb of one trace, walking the program once:
+// records of other constraints are skipped, a constraint without records gets zeros.  x_m and iz_m are the plan's x_i
+// and 1/Z_i, cur and nxt the trace's nregs rows T_s(x_i) and nregs rows T_s(step * x_i) (canonical); coefficients are
+// canonical, so a coefficient times a Montgomery-form power is canonical again  (i < n)
+SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *cur, const fe *nxt,
+                         long long c0, long long nb, int nregs, int log_n, long long i) {
     const long long n = 1ll << log_n;
     const fe x = tile_ld(x_m + i), iz = tile_ld(iz_m + i), h0 = tile_ldg(prog);
     const long long nrec = (long long)h0.v[0] | (long long)h0.v[1] << 32, stride = 2 + (nregs + 1) / 2;
-    long long cur = c0;
+    long long c_at = c0;
     fe acc = fe_zero(), s = fe_zero(), xp = fe_mont_one();
     for (long long t = 0; t < nrec; t++) {
         const fe *rec = prog + 1 + t * stride;
@@ -74,7 +78,7 @@ SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, c
         const long long c = h.v[0];
         if (c < c0) continue;
         if (c >= c0 + nb) break;
-        for (; cur < c; cur++, acc = fe_zero()) tile_st(V + (cur - c0) * n + i, fe_montmul(acc, iz));
+        for (; c_at < c; c_at++, acc = fe_zero()) tile_st(V + (c_at - c0) * n + i, fe_montmul(acc, iz));
         if (h.v[1] & AIR_FIRST) {
             xp = air_pow(x, h.v[2]);
             s = fe_zero();
@@ -87,14 +91,34 @@ SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, c
                 const fe e4 = tile_ldg(rec + 2 + w);
                 for (int k = 0; k < 4; k++) {
                     const int v = 4 * w + k;
-                    if (v < 2 * nregs && e4.v[k])
-                        s = fe_montmul(s, air_pow(fe_to_mont(tile_ld(ext + v * n + i)), e4.v[k]));
+                    if (v < 2 * nregs && e4.v[k]) {
+                        const fe *row = v < nregs ? cur + v * n : nxt + (v - nregs) * n;
+                        s = fe_montmul(s, air_pow(fe_to_mont(tile_ld(row + i)), e4.v[k]));
+                    }
                 }
             }
             acc = fe_add(acc, s);
         }
     }
-    for (; cur < c0 + nb; cur++, acc = fe_zero()) tile_st(V + (cur - c0) * n + i, fe_montmul(acc, iz));
+    for (; c_at < c0 + nb; c_at++, acc = fe_zero()) tile_st(V + (c_at - c0) * n + i, fe_montmul(acc, iz));
+}
+// the same for one trace whose 2 nregs rows lie together: current rows at ext, next rows at ext + nregs n
+SA_HD void air_eval_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long c0,
+                         long long nb, int nregs, int log_n, long long i) {
+    air_eval_elem(V, prog, x_m, iz_m, ext, ext + ((long long)nregs << log_n), c0, nb, nregs, log_n, i);
+}
+// The rows r0 <= r < r0 + nb of a chunk of bp traces, row r = b * ncons + c being trace b's constraint c:
+// air_eval_elem once per trace the rows touch, trace b's current rows at ext + b nregs n and its next rows at
+// ext + (bp + b) nregs n (the chunk's two coset loads, each of bp * nregs rows)  (i < n)
+SA_HD void air_eval_rows_elem(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long r0,
+                              long long nb, long long ncons, long long bp, int nregs, int log_n, long long i) {
+    const long long n = 1ll << log_n, rows = (long long)nregs * n;
+    for (long long b = r0 / ncons; b * ncons < r0 + nb; b++) {
+        const long long lo = r0 > b * ncons ? r0 : b * ncons;
+        const long long hi = r0 + nb < (b + 1) * ncons ? r0 + nb : (b + 1) * ncons;
+        air_eval_elem(V + (lo - r0) * n, prog, x_m, iz_m, ext + b * rows, ext + (bp + b) * rows, lo - b * ncons,
+                      hi - lo, nregs, log_n, i);
+    }
 }
 
 // ---- element function: the body of k_air_store_exact ----
@@ -145,11 +169,31 @@ inline AirPlan air_plan_layout(int log_n, size_t max_ncoef, size_t nregs, size_t
     return L;
 }
 
-// An apply's workspace: the 2 nregs transformed rows and n elements per constraint row of a chunk (its chunks are
-// coset_batch_max(log_n) constraints); the transforms take the NTT's own besides.
+// A batched apply runs in chunks of whole traces, and within a chunk in row chunks of the chunk's bp * ncons
+// constraint rows.  A chunk takes 2 nregs transformed rows per trace and n elements per row of a row chunk: 16 bytes
+// per element of its own workspace and 16 of the transform's, 32 n bytes per row, as coset_batch_max counts them.  So
+// a chunk holds as many traces as keep its 2 nregs + ncons rows per trace within coset_batch_max(log_n) rows (1 GiB),
+// at least one, and a row chunk at most coset_batch_max(log_n) rows: a chunk of several traces is then one row chunk
+// and issues the launches of one trace's apply, and a batch of one is chunked as the single apply always was.
+struct AirChunks {
+    size_t traces = 0, rows = 0;
+};
 inline size_t air_chunk(size_t ncons, int log_n) { return std::min(ncons, coset_batch_max(log_n)); }
+inline size_t air_batch_max(size_t nregs, size_t ncons, int log_n) {
+    const size_t cap = coset_batch_max(log_n), per = 2 * nregs + ncons;
+    return cap == 0 ? 0 : std::max<size_t>(1, cap / per);
+}
+inline AirChunks air_chunks(size_t nregs, size_t ncons, size_t batch, int log_n) {
+    AirChunks k;
+    k.traces = std::max<size_t>(1, std::min(batch, air_batch_max(nregs, ncons, log_n)));
+    k.rows = air_chunk(k.traces * ncons, log_n);
+    return k;
+}
+inline size_t air_ws_elems(size_t nregs, const AirChunks &k, int log_n) {
+    return ((size_t)1 << log_n) * (2 * nregs * k.traces + k.rows);
+}
 inline size_t air_ws_elems(size_t nregs, size_t ncons, int log_n) {
-    return ((size_t)1 << log_n) * (2 * nregs + air_chunk(ncons, log_n));
+    return air_ws_elems(nregs, air_chunks(nregs, ncons, 1, log_n), log_n);
 }
 
 // ---- checks, before any workspace is taken and before any launch ----
@@ -235,49 +279,87 @@ int air_plan_build(B &b, fe *plan, const std::vector<fe> &prog, const fe *zerofi
     return b.upload(plan + L.prog, prog.data(), prog.size());
 }
 
-// The quotients of the plan's constraints for trace[nregs][ncoef] (coefficient rows): out[ncons][qlen].  The current
-// rows loaded with offset^i and the next rows with (offset * step)^j, one batched forward transform of the 2 nregs
-// rows, then per chunk of coset_batch_max(log_n) constraints k_air_eval, one batched inverse transform and
-// store(c0, nb, V), the chunk's store from V: 3 + 3 ceil(ncons / chunk) launches plus the transforms', whatever nregs
-// and the chunk's size.  ws = air_ws_elems(nregs, ncons, log_n) elements.
+// The quotients of the plan's constraints for `batch` traces trace[batch][nregs][ncoef] (coefficient rows):
+// out[batch][ncons][qlen], trace b's rows exactly the apply of trace b alone.  Per chunk of k.traces traces: the
+// current rows of its traces loaded with offset^i and the next rows with (offset * step)^j, one batched forward
+// transform of the 2 nregs rows per trace, then per row chunk of k.rows constraint rows k_air_eval, one batched
+// inverse transform and store(r, nb, V), the store of rows r .. r + nb of out from V: 3 + 3 ceil(ncons / k.rows)
+// launches per chunk plus the transforms', whatever nregs and the chunk's size.  ws = air_ws_elems(nregs, k, log_n)
+// elements.  The library takes k = air_chunks(...); the emulation may take smaller chunks.
+// b.air_eval: a backend's k_air_eval over the rows of a chunk of bp traces (air_eval_rows_elem).  A backend whose
+// air_eval takes one trace's rows, (V, prog, x, iz, ext, c0, nb, nregs, log_n) as air_eval_elem does, serves chunks
+// of one trace, the only chunks a batch of one makes.
+template <class B>
+auto air_eval_call(B &b, fe *V, const fe *prog, const fe *x, const fe *iz, const fe *ext, long long r0, long long nb,
+                   long long ncons, long long bp, int nregs, int log_n, int)
+    -> decltype(b.air_eval(V, prog, x, iz, ext, r0, nb, ncons, bp, nregs, log_n)) {
+    return b.air_eval(V, prog, x, iz, ext, r0, nb, ncons, bp, nregs, log_n);
+}
+template <class B>
+int air_eval_call(B &b, fe *V, const fe *prog, const fe *x, const fe *iz, const fe *ext, long long r0, long long nb,
+                  long long /*ncons*/, long long bp, int nregs, int log_n, long) {
+    return bp == 1 ? b.air_eval(V, prog, x, iz, ext, r0, nb, nregs, log_n) : SA_ESIZE;
+}
+
 template <class B, class Store>
-int air_apply(B &b, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t ncons, int log_n,
-              const uint64_t root[2], fe *ws, Store store) {
+int air_apply(B &b, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t ncons, size_t batch,
+              int log_n, const uint64_t root[2], fe *ws, const AirChunks &k, Store store) {
     const AirPlan L = air_plan_layout(log_n, 1, nregs, 0);
-    const long long n = L.n;
-    fe *ext = ws, *V = ws + 2 * nregs * (size_t)n;
-    SA_TRY(b.coset_load(ext, trace, plan + L.div.pw, (long long)ncoef, log_n, (long long)nregs));
-    SA_TRY(b.coset_load(ext + nregs * (size_t)n, trace, plan + L.spw, (long long)ncoef, log_n, (long long)nregs));
-    SA_TRY(b.ntt(ext, ext, log_n, root, 0, 2 * nregs));
-    const size_t chunk = air_chunk(ncons, log_n);
-    for (size_t c0 = 0; c0 < ncons; c0 += chunk) {
-        const size_t nb = std::min(chunk, ncons - c0);
-        SA_TRY(b.air_eval(V, plan + L.prog, plan + L.x, plan + L.div.inv, ext, (long long)c0, (long long)nb,
-                          (int)nregs, log_n));
-        SA_TRY(b.ntt(V, V, log_n, root, 1, nb));
-        SA_TRY(store(c0, nb, V));
+    const size_t n = (size_t)L.n;
+    for (size_t p0 = 0; p0 < batch; p0 += k.traces) {
+        const size_t bp = std::min(k.traces, batch - p0), rows = bp * ncons;
+        const fe *tr = trace + p0 * nregs * ncoef;
+        fe *ext = ws, *V = ws + 2 * nregs * bp * n;
+        SA_TRY(b.coset_load(ext, tr, plan + L.div.pw, (long long)ncoef, log_n, (long long)(bp * nregs)));
+        SA_TRY(b.coset_load(ext + bp * nregs * n, tr, plan + L.spw, (long long)ncoef, log_n, (long long)(bp * nregs)));
+        SA_TRY(b.ntt(ext, ext, log_n, root, 0, 2 * bp * nregs));
+        for (size_t r0 = 0; r0 < rows; r0 += k.rows) {
+            const size_t nb = std::min(k.rows, rows - r0);
+            SA_TRY(air_eval_call(b, V, plan + L.prog, plan + L.x, plan + L.div.inv, ext, (long long)r0,
+                                 (long long)nb, (long long)ncons, (long long)bp, (int)nregs, log_n, 0));
+            SA_TRY(b.ntt(V, V, log_n, root, 1, nb));
+            SA_TRY(store(p0 * ncons + r0, nb, V));
+        }
     }
     return SA_OK;
 }
-// the apply: k_coset_store per chunk
+// the apply: k_coset_store per row chunk
+template <class B>
+int air_quotients(B &b, fe *out, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t qlen,
+                  size_t ncons, size_t batch, int log_n, const uint64_t root[2], fe *ws, const AirChunks &k) {
+    const fe *ipw = plan + air_plan_layout(log_n, 1, nregs, 0).div.ipw;
+    return air_apply(b, plan, trace, nregs, ncoef, ncons, batch, log_n, root, ws, k,
+                     [&](size_t r, size_t nb, const fe *V) {
+                         return b.coset_store(out + r * qlen, V, ipw, (long long)qlen, log_n, (long long)nb);
+                     });
+}
+// the exact apply: the flags[batch][ncons] cleared first, then k_air_store_exact per row chunk -- the apply's
+// launches plus one
+template <class B>
+int air_quotients_exact(B &b, fe *out, uint32_t *flags, const fe *plan, const fe *trace, size_t nregs, size_t ncoef,
+                        size_t qlen, size_t ncons, size_t batch, size_t tail, int log_n, const uint64_t root[2],
+                        fe *ws, const AirChunks &k) {
+    const fe *ipw = plan + air_plan_layout(log_n, 1, nregs, 0).div.ipw;
+    SA_TRY(b.clear_flags(flags, batch * ncons));
+    return air_apply(b, plan, trace, nregs, ncoef, ncons, batch, log_n, root, ws, k,
+                     [&](size_t r, size_t nb, const fe *V) {
+                         return b.air_store_exact(out + r * qlen, flags + r, V, ipw, (long long)qlen, (long long)tail,
+                                                  log_n, (long long)nb);
+                     });
+}
+
+// the single-trace applies: batch 1 of the schedules above, with the library's chunks
 template <class B>
 int air_quotients(B &b, fe *out, const fe *plan, const fe *trace, size_t nregs, size_t ncoef, size_t qlen,
                   size_t ncons, int log_n, const uint64_t root[2], fe *ws) {
-    const fe *ipw = plan + air_plan_layout(log_n, 1, nregs, 0).div.ipw;
-    return air_apply(b, plan, trace, nregs, ncoef, ncons, log_n, root, ws, [&](size_t c0, size_t nb, const fe *V) {
-        return b.coset_store(out + c0 * qlen, V, ipw, (long long)qlen, log_n, (long long)nb);
-    });
+    return air_quotients(b, out, plan, trace, nregs, ncoef, qlen, ncons, 1, log_n, root, ws,
+                         air_chunks(nregs, ncons, 1, log_n));
 }
-// the exact apply: the flags[ncons] cleared first, then k_air_store_exact per chunk -- the apply's launches plus one
 template <class B>
 int air_quotients_exact(B &b, fe *out, uint32_t *flags, const fe *plan, const fe *trace, size_t nregs, size_t ncoef,
                         size_t qlen, size_t ncons, size_t tail, int log_n, const uint64_t root[2], fe *ws) {
-    const fe *ipw = plan + air_plan_layout(log_n, 1, nregs, 0).div.ipw;
-    SA_TRY(b.clear_flags(flags, ncons));
-    return air_apply(b, plan, trace, nregs, ncoef, ncons, log_n, root, ws, [&](size_t c0, size_t nb, const fe *V) {
-        return b.air_store_exact(out + c0 * qlen, flags + c0, V, ipw, (long long)qlen, (long long)tail, log_n,
-                                 (long long)nb);
-    });
+    return air_quotients_exact(b, out, flags, plan, trace, nregs, ncoef, qlen, ncons, 1, tail, log_n, root, ws,
+                               air_chunks(nregs, ncons, 1, log_n));
 }
 
 }  // namespace sa

@@ -39,34 +39,41 @@ SA_HD void coset_store_elem(fe *out, const fe *ws, const fe *ipw_m, long long ql
     if (j < qlen) tile_st(out + b * qlen + j, fe_montmul(tile_ld(ws + idx), tile_ld(ipw_m + j)));
 }
 
-// A group of a combination's terms, taken by one launch as a kernel parameter (__grid_constant__: 2.5 KB, inside the
+// A group of a combination's terms, taken by one launch as a kernel parameter (__grid_constant__: 3 KB, inside the
 // classic 4 KB parameter limit).  Term t is the row src[0..len) shifted up by `shift`, weighted by w_m (Montgomery
-// form, so each covered index costs one fe_montmul and one fe_add).
+// form, so each covered index costs one fe_montmul and one fe_add), and added into destination row `row`.
 constexpr int COMBINE_TERMS = 64;
 struct CombineTerm {
     const fe *src;
-    long long len, shift;
+    long long len, shift, row;
     fe w_m;
 };
 struct CombineGroup {
     CombineTerm t[COMBINE_TERMS];
     int count;
 };
-// out[i] (+)= offset^i * sum_t w_t * src_t[i - shift_t] over the group's terms whose window covers i, for i < ncomb;
-// the first group (first != 0) writes every i < n, zero from ncomb on, each later one adds its own scaled sum
-// (scaling by offset^i is linear)  (idx < n)
-SA_HD void coset_combine_elem(fe *out, const CombineGroup &g, const fe *pw_m, long long ncomb, int first, long long i) {
+// out[r][i] (+)= offset^i * sum_t w_t * src_t[i - shift_t] over the group's terms of row r whose window covers i, for
+// i < ncomb (the longest row's length; a shorter row's sum is zero past its own); the first group (first != 0)
+// writes every i < n of every row, zero from ncomb on, each later one adds its own scaled sum (scaling by offset^i is
+// linear)  (idx = r * n + i < nrows * n)
+SA_HD void coset_combine_elem(fe *out, const CombineGroup &g, const fe *pw_m, long long ncomb, int first, int log_n,
+                              long long idx) {
+    const long long r = idx >> log_n, i = idx & ((1ll << log_n) - 1);
     if (i >= ncomb) {
-        if (first) tile_st(out + i, fe_zero());
+        if (first) tile_st(out + idx, fe_zero());
         return;
     }
     fe s = fe_zero();
     for (int t = 0; t < g.count; t++) {
         const long long j = i - g.t[t].shift;
-        if (j >= 0 && j < g.t[t].len) s = fe_add(s, fe_montmul(tile_ld(g.t[t].src + j), g.t[t].w_m));
+        if (g.t[t].row == r && j >= 0 && j < g.t[t].len) s = fe_add(s, fe_montmul(tile_ld(g.t[t].src + j), g.t[t].w_m));
     }
     s = fe_montmul(s, tile_ld(pw_m + i));
-    tile_st(out + i, first ? s : fe_add(tile_ld(out + i), s));
+    tile_st(out + idx, first ? s : fe_add(tile_ld(out + idx), s));
+}
+// one row: out[i] for i < n, every term in row 0
+SA_HD void coset_combine_elem(fe *out, const CombineGroup &g, const fe *pw_m, long long ncomb, int first, long long i) {
+    coset_combine_elem(out, g, pw_m, ncomb, first, 62, i);
 }
 
 // ---- host schedule ----
@@ -176,26 +183,48 @@ inline size_t coset_combine_len(const size_t *lens, const size_t *shifts, size_t
     return m;
 }
 // the checks of a combination, before its workspace is taken and before its first launch: the size, every term's
-// window inside [0, n) and the root (sa_ntt's SA_EROOTORDER / SA_ENOTPRIM).  Every offset is accepted, 0 included.
-inline int coset_combine_check(int log_n, const size_t *lens, const size_t *shifts, size_t nterms,
-                               const uint64_t root[2]) {
+// window inside [0, n), every term's destination row below nrows (rows == nullptr: every term in row 0) and the root
+// (sa_ntt's SA_EROOTORDER / SA_ENOTPRIM).  Every offset is accepted, 0 included.
+inline int coset_combine_check(int log_n, const size_t *lens, const size_t *shifts, const size_t *rows, size_t nrows,
+                               size_t nterms, const uint64_t root[2]) {
     if (log_n < 1 || log_n > COSET_MAX_LOG) return SA_ESIZE;
     const size_t n = (size_t)1 << log_n;
     for (size_t t = 0; t < nterms; t++)
-        if (shifts[t] > n || lens[t] > n - shifts[t]) return SA_ESIZE;
+        if (shifts[t] > n || lens[t] > n - shifts[t] || (rows ? rows[t] : 0) >= nrows) return SA_ESIZE;
     return ntt_check_root(fe_to_mont(fe_from_limbs(root)), log_n);
 }
 
-// out = ntt(c[i] * offset^i, zero padded to n), c[i] = sum_t w_t * srcs[t][i - shifts[t]] over the terms with
-// shifts[t] <= i < shifts[t] + lens[t] (fast_coset_evaluate of the combination at order n): offset^i for i < ncomb
-// into pw (ncomb elements), then the terms in groups of COMBINE_TERMS, one launch each (the first writes all of out,
-// the others add), then one transform in place -- 1 + ceil(nterms / 64) launches plus the transform's.  With
-// ncomb == 0 (no term, or only empty ones at shift 0) out is n zeros from the group launches alone: no table, no
-// transform.  out must not overlap any source.
+// one row's: every term in row 0
+inline int coset_combine_check(int log_n, const size_t *lens, const size_t *shifts, size_t nterms,
+                               const uint64_t root[2]) {
+    return coset_combine_check(log_n, lens, shifts, nullptr, 1, nterms, root);
+}
+
+// b.coset_combine: a backend's k_coset_combine over nrows rows.  A backend whose coset_combine takes one row, (out,
+// g, pw, ncomb, log_n, first), serves nrows == 1.
 template <class B>
-int coset_combine_evaluate(B &b, fe *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
-                           const fe *const *srcs, const size_t *lens, const size_t *shifts, const uint64_t *weights,
-                           size_t nterms, fe *pw) {
+auto coset_combine_call(B &b, fe *out, const CombineGroup &g, const fe *pw, long long ncomb, int log_n,
+                        long long nrows, int first, int) -> decltype(b.coset_combine(out, g, pw, ncomb, log_n, nrows,
+                                                                                     first)) {
+    return b.coset_combine(out, g, pw, ncomb, log_n, nrows, first);
+}
+template <class B>
+int coset_combine_call(B &b, fe *out, const CombineGroup &g, const fe *pw, long long ncomb, int log_n, long long nrows,
+                       int first, long) {
+    return nrows == 1 ? b.coset_combine(out, g, pw, ncomb, log_n, first) : SA_ESIZE;
+}
+
+// out[r] = ntt(c_r[i] * offset^i, zero padded to n) for r < nrows, c_r[i] = sum_t w_t * srcs[t][i - shifts[t]] over
+// the terms of row r (rows[t] == r; rows == nullptr puts every term in row 0) with shifts[t] <= i < shifts[t] +
+// lens[t] (fast_coset_evaluate of each row's combination at order n): offset^i for i < ncomb into pw (ncomb elements,
+// the longest row's), then the terms in groups of COMBINE_TERMS, one launch each over all rows (the first writes all
+// of out, the others add), then one batched transform of the nrows rows in place -- 1 + ceil(nterms / 64) launches
+// plus the transform's, whatever nrows.  With ncomb == 0 (no term, or only empty ones at shift 0) out is zeros from
+// the group launches alone: no table, no transform.  out must not overlap any source.  nrows >= 1.
+template <class B>
+int coset_combine_evaluate(B &b, fe *out, size_t nrows, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                           const fe *const *srcs, const size_t *lens, const size_t *shifts, const size_t *rows,
+                           const uint64_t *weights, size_t nterms, fe *pw) {
     const long long ncomb = (long long)coset_combine_len(lens, shifts, nterms);
     if (ncomb) SA_TRY(b.pow_table(pw, fe_to_mont(fe_from_limbs(offset)), ncomb));
     for (size_t t0 = 0; t0 == 0 || t0 < nterms; t0 += COMBINE_TERMS) {
@@ -203,10 +232,18 @@ int coset_combine_evaluate(B &b, fe *out, int log_n, const uint64_t root[2], con
         g.count = (int)std::min((size_t)COMBINE_TERMS, nterms - t0);
         for (int k = 0; k < g.count; k++)
             g.t[k] = CombineTerm{srcs[t0 + k], (long long)lens[t0 + k], (long long)shifts[t0 + k],
-                                 fe_to_mont(fe_from_limbs(weights + 2 * (t0 + k)))};
-        SA_TRY(b.coset_combine(out, g, pw, ncomb, log_n, t0 == 0));
+                                 rows ? (long long)rows[t0 + k] : 0, fe_to_mont(fe_from_limbs(weights + 2 * (t0 + k)))};
+        SA_TRY(coset_combine_call(b, out, g, pw, ncomb, log_n, (long long)nrows, t0 == 0, 0));
     }
-    return ncomb ? b.ntt(out, out, log_n, root, 0, 1) : SA_OK;
+    return ncomb ? b.ntt(out, out, log_n, root, 0, nrows) : SA_OK;
+}
+
+// one combination: nrows = 1 of the schedule above, every term in row 0
+template <class B>
+int coset_combine_evaluate(B &b, fe *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                           const fe *const *srcs, const size_t *lens, const size_t *shifts, const uint64_t *weights,
+                           size_t nterms, fe *pw) {
+    return coset_combine_evaluate(b, out, 1, log_n, root, offset, srcs, lens, shifts, nullptr, weights, nterms, pw);
 }
 
 }  // namespace sa

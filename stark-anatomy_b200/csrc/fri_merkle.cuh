@@ -3,10 +3,13 @@
 // __host__ __device__ so tests/emu can drive the same code phase by phase; the launch loop of a tree
 // and the fold scalars are shared with it too.
 #pragma once
+#include <algorithm>
 #include <cstdio>
 
 #include "field.cuh"
 #include "hash.cuh"
+#include "host.cuh"
+#include "ntt_tile.cuh"
 
 namespace sa {
 
@@ -213,6 +216,36 @@ SA_HD void merkle_private(uint64_t root[8], const MerkleArgs &a, long long blk, 
             for (int i = 0; i < 8; i++) slot[h][i] = d[i];
     }
     for (int i = 0; i < 8; i++) root[i] = d[i];
+}
+
+// ---- openings with an index set per group: sa_gather_batch_sets and sa_merkle_open_batch_sets ----
+// Rows (trees) are taken in groups of `group`; row b reads set b / group, indices[(b / group) * k .. + k).  The
+// ungrouped calls are group = batch: every row reads the one set.
+// the number of indices the sets of a call hold, ceil(batch / group) sets of k and at least one (a call without rows
+// still checks its indices), after checking them: SA_ESIZE for group == 0, SA_EINDEX for any index >= n
+inline int index_sets_check(const uint64_t *indices, size_t batch, size_t group, size_t k, size_t n, size_t *count) {
+    if (group == 0) return SA_ESIZE;
+    *count = std::max<size_t>(1, (batch + group - 1) / group) * k;
+    for (size_t i = 0; i < *count; i++)
+        if (indices[i] >= n) return SA_EINDEX;
+    return SA_OK;
+}
+// out[b][q] = values[b * n + the index q of row b's set]  (t = b * k + q < batch * k)
+SA_HD void gather_sets_elem(fe *out, const fe *values, long long n, const uint64_t *indices, long long k,
+                            long long group, long long t) {
+    const long long b = t / k, q = t - b * k;
+    tile_st(out + t, tile_ld(values + b * n + (long long)indices[(b / group) * k + q]));
+}
+// out[b][q][level] = word w of the sibling at `level` of the leaf index q of tree b's set, in tree b (trees 2n nodes
+// apart)  (t = ((b * k + q) * depth + level) * 8 + w < batch * k * depth * 8)
+SA_HD void merkle_path_sets_elem(uint64_t *out, const uint64_t *trees, long long n, int depth, const uint64_t *indices,
+                                 long long k, long long group, long long t) {
+    const int w = (int)(t & 7);
+    const long long ql = t >> 3;
+    const int level = (int)(ql % depth);
+    const long long qb = ql / depth, q = qb % k, b = qb / k;
+    const long long node = ((n + (long long)indices[(b / group) * k + q]) >> level) ^ 1;
+    out[t] = trees[(b * 2 * n + node) * 8 + w];
 }
 
 }  // namespace sa

@@ -126,24 +126,17 @@ __global__ void __launch_bounds__(MK_THREADS, 2) k_merkle_chunk(const __grid_con
     if (a.root_out && tid == 0) merkle_publish_root(a, sm);
 }
 
-// out[b][q][level] = word w of the sibling at `level` of leaf indices[q] in tree b (trees 2n nodes apart)
+// out[b][q][level] = word w of the sibling at `level` of the leaf index q of tree b's set, in tree b
 __global__ void k_merkle_paths(uint64_t *out, const uint64_t *trees, long long n, int depth,
-                               const uint64_t *indices, long long k, long long batch) {
+                               const uint64_t *indices, long long k, long long batch, long long group) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = batch * k * depth * 8;
-    if (t >= total) return;
-    const int w = (int)(t & 7);
-    const long long ql = t >> 3;
-    const int level = (int)(ql % depth);
-    const long long qb = ql / depth, q = qb % k, b = qb / k;
-    const long long node = ((n + (long long)indices[q]) >> level) ^ 1;
-    out[t] = trees[(b * 2 * n + node) * 8 + w];
+    if (t < batch * k * depth * 8) merkle_path_sets_elem(out, trees, n, depth, indices, k, group, t);
 }
-// out[b][q] = values[b * n + indices[q]]
+// out[b][q] = values[b * n + the index q of row b's set]
 __global__ void k_gather(fe *out, const fe *values, long long n, const uint64_t *indices, long long k,
-                         long long batch) {
+                         long long batch, long long group) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < batch * k) tile_st(out + t, tile_ld(values + (t / k) * n + indices[t % k]));
+    if (t < batch * k) gather_sets_elem(out, values, n, indices, k, group, t);
 }
 
 // blake2b-only roof of the Merkle kernels: every thread hashes a chain of node messages (128 bytes = one
@@ -272,35 +265,41 @@ int sa_merkle_tree(void *tree, const void *values, size_t n, void *stream) {
     return sa_merkle_tree_batch(tree, values, n, 1, stream);
 }
 
-// checks the k leaf indices against n and, when the call has work (`work`, k > 0), uploads them to
+// checks the index sets (index_sets_check) and, when the call has work (`work`, k > 0), uploads them to
 // stream-ordered device memory; *idx stays nullptr otherwise
-static int upload_indices(uint64_t **idx, const uint64_t *indices_host, size_t k, size_t n, bool work,
-                          cudaStream_t st) {
-    for (size_t i = 0; i < k; i++)
-        if (indices_host[i] >= n) return SA_EINDEX;
+static int upload_indices(uint64_t **idx, const uint64_t *indices_host, size_t batch, size_t group, size_t k, size_t n,
+                          bool work, cudaStream_t st) {
+    size_t count = 0;
+    SA_TRY(index_sets_check(indices_host, batch, group, k, n, &count));
     *idx = nullptr;
-    if (!work || k == 0) return SA_OK;
+    if (!work || count == 0) return SA_OK;
     keep_pool_memory();
-    SA_CUDA(cudaMallocAsync((void **)idx, 8 * k, st));
-    SA_CUDA(cudaMemcpyAsync(*idx, indices_host, 8 * k, cudaMemcpyHostToDevice, st));
+    SA_CUDA(cudaMallocAsync((void **)idx, 8 * count, st));
+    SA_CUDA(cudaMemcpyAsync(*idx, indices_host, 8 * count, cudaMemcpyHostToDevice, st));
+    return SA_OK;
+}
+
+int sa_merkle_open_batch_sets(void *paths_out, const void *trees, size_t n, size_t batch, size_t group,
+                              const uint64_t *indices_host, size_t k, void *stream) {
+    if (!host_is_pow2(n)) return SA_ENOTPOW2;
+    const int depth = host_log2(n);
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t *idx = nullptr;
+    int rc = upload_indices(&idx, indices_host, batch, group, k, n, batch != 0 && depth != 0, st);
+    if (rc != SA_OK || idx == nullptr) return rc;
+    const long long total = (long long)batch * (long long)k * depth * 8;
+    k_merkle_paths<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((uint64_t *)paths_out,
+                                                                    (const uint64_t *)trees, (long long)n,
+                                                                    depth, idx, (long long)k, (long long)batch,
+                                                                    (long long)group);
+    SA_LAUNCH_CHECK();
+    cudaFreeAsync(idx, st);
     return SA_OK;
 }
 
 int sa_merkle_open_batch(void *paths_out, const void *trees, size_t n, size_t batch, const uint64_t *indices_host,
                          size_t k, void *stream) {
-    if (!host_is_pow2(n)) return SA_ENOTPOW2;
-    const int depth = host_log2(n);
-    cudaStream_t st = (cudaStream_t)stream;
-    uint64_t *idx = nullptr;
-    int rc = upload_indices(&idx, indices_host, k, n, batch != 0 && depth != 0, st);
-    if (rc != SA_OK || idx == nullptr) return rc;
-    const long long total = (long long)batch * (long long)k * depth * 8;
-    k_merkle_paths<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((uint64_t *)paths_out,
-                                                                    (const uint64_t *)trees, (long long)n,
-                                                                    depth, idx, (long long)k, (long long)batch);
-    SA_LAUNCH_CHECK();
-    cudaFreeAsync(idx, st);
-    return SA_OK;
+    return sa_merkle_open_batch_sets(paths_out, trees, n, batch, batch ? batch : 1, indices_host, k, stream);
 }
 
 int sa_merkle_open(void *paths_out, const void *tree, size_t n, const uint64_t *indices_host, size_t k,
@@ -308,18 +307,23 @@ int sa_merkle_open(void *paths_out, const void *tree, size_t n, const uint64_t *
     return sa_merkle_open_batch(paths_out, tree, n, 1, indices_host, k, stream);
 }
 
-int sa_gather_batch(void *out, const void *values, size_t n, size_t batch, const uint64_t *indices_host, size_t k,
-                    void *stream) {
+int sa_gather_batch_sets(void *out, const void *values, size_t n, size_t batch, size_t group,
+                         const uint64_t *indices_host, size_t k, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     uint64_t *idx = nullptr;
-    int rc = upload_indices(&idx, indices_host, k, n, batch != 0, st);
+    int rc = upload_indices(&idx, indices_host, batch, group, k, n, batch != 0, st);
     if (rc != SA_OK || idx == nullptr) return rc;
     const long long total = (long long)batch * (long long)k;
     k_gather<<<(unsigned)((total + 127) / 128), 128, 0, st>>>((fe *)out, (const fe *)values, (long long)n, idx,
-                                                            (long long)k, (long long)batch);
+                                                            (long long)k, (long long)batch, (long long)group);
     SA_LAUNCH_CHECK();
     cudaFreeAsync(idx, st);
     return SA_OK;
+}
+
+int sa_gather_batch(void *out, const void *values, size_t n, size_t batch, const uint64_t *indices_host, size_t k,
+                    void *stream) {
+    return sa_gather_batch_sets(out, values, n, batch, batch ? batch : 1, indices_host, k, stream);
 }
 
 int sa_gather(void *out, const void *values, size_t n, const uint64_t *indices_host, size_t k, void *stream) {

@@ -211,15 +211,17 @@ __global__ void k_coset_quot(fe *ws, const fe *inv_m, int log_n, long long batch
 __global__ void k_coset_store(fe *out, const fe *ws, const fe *ipw_m, long long qlen, int log_n, long long batch) {
     grid_stride(batch << log_n, [&](long long idx) { coset_store_elem(out, ws, ipw_m, qlen, log_n, idx); });
 }
-// one group of a combination's terms over all n outputs; the group is a kernel parameter, so the call uploads nothing
+// one group of a combination's terms over all nrows * n outputs; the group is a kernel parameter, so the call uploads
+// nothing
 __global__ void k_coset_combine(fe *out, const __grid_constant__ CombineGroup g, const fe *pw_m, long long ncomb,
-                                int log_n, int first) {
-    grid_stride(1ll << log_n, [&](long long i) { coset_combine_elem(out, g, pw_m, ncomb, first, i); });
+                                int log_n, long long nrows, int first) {
+    grid_stride(nrows << log_n, [&](long long idx) { coset_combine_elem(out, g, pw_m, ncomb, first, log_n, idx); });
 }
-// the quotient values of nb constraints, one thread per point
-__global__ void k_air_eval(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long c0,
-                           long long nb, int nregs, int log_n) {
-    grid_stride(1ll << log_n, [&](long long i) { air_eval_elem(V, prog, x_m, iz_m, ext, c0, nb, nregs, log_n, i); });
+// the quotient values of nb constraint rows of a chunk of bp traces, one thread per point
+__global__ void k_air_eval(fe *V, const fe *prog, const fe *x_m, const fe *iz_m, const fe *ext, long long r0,
+                           long long nb, long long ncons, long long bp, int nregs, int log_n) {
+    grid_stride(1ll << log_n,
+                [&](long long i) { air_eval_rows_elem(V, prog, x_m, iz_m, ext, r0, nb, ncons, bp, nregs, log_n, i); });
 }
 // the boundary quotient codewords of batch registers in place, one thread per point
 __global__ void k_boundary_point(fe *cw, const fe *ival, const fe *izinv_m, long long stride, int log_n,
@@ -325,8 +327,8 @@ struct DeviceTree {
     int coset_store(fe *o, const fe *ws, const fe *ipw, ll q, int lg, ll nb) {
         return go(k_coset_store, tree_grid(nb << lg), o, ws, ipw, q, lg, nb);
     }
-    int coset_combine(fe *o, const CombineGroup &g, const fe *pw, ll nc, int lg, int first) {
-        return go(k_coset_combine, tree_grid(1ll << lg), o, g, pw, nc, lg, first);
+    int coset_combine(fe *o, const CombineGroup &g, const fe *pw, ll nc, int lg, ll nrows, int first) {
+        return go(k_coset_combine, tree_grid(nrows << lg), o, g, pw, nc, lg, nrows, first);
     }
     int ntt(fe *o, const fe *i, int lg, const uint64_t *r, int inv, size_t nb) { return sa_ntt(o, i, lg, r, inv, nb, st); }
     int copy(fe *dst, const fe *src, size_t n) {
@@ -352,8 +354,9 @@ struct DeviceAir : DeviceTree {
         SA_CUDA(cudaMemcpyAsync(dst, src, sizeof(fe) * n, cudaMemcpyHostToDevice, st));
         return SA_OK;
     }
-    int air_eval(fe *V, const fe *prog, const fe *x, const fe *iz, const fe *ext, ll c0, ll nb, int nregs, int lg) {
-        return go(k_air_eval, tree_grid(1ll << lg), V, prog, x, iz, ext, c0, nb, nregs, lg);
+    int air_eval(fe *V, const fe *prog, const fe *x, const fe *iz, const fe *ext, ll r0, ll nb, ll ncons, ll bp,
+                 int nregs, int lg) {
+        return go(k_air_eval, tree_grid(1ll << lg), V, prog, x, iz, ext, r0, nb, ncons, bp, nregs, lg);
     }
 };
 // DeviceAir (its upload) plus the copies and launches only the boundary schedules make (boundary.cuh)
@@ -573,17 +576,26 @@ int sa_coset_evaluate_batch(void *out, const void *coeffs, size_t ncoef, int log
 }
 
 // scratch: offset^i for i < ncomb (WS_COSET); the terms travel as kernel parameters and out is transformed in place
-int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
-                              const void *const *srcs, const size_t *lens, const size_t *shifts,
-                              const uint64_t *weights, size_t nterms, void *stream) {
-    SA_TRY(coset_combine_check(log_n, lens, shifts, nterms, root));
+int sa_coset_combine_evaluate_batch(void *out, size_t nrows, int log_n, const uint64_t root[2],
+                                    const uint64_t offset[2], const void *const *srcs, const size_t *lens,
+                                    const size_t *shifts, const size_t *rows, const uint64_t *weights, size_t nterms,
+                                    void *stream) {
+    SA_TRY(coset_combine_check(log_n, lens, shifts, rows, nrows, nterms, root));
+    if (nrows == 0) return SA_OK;
     cudaStream_t st = (cudaStream_t)stream;
     fe *pw = nullptr;
     const size_t ncomb = coset_combine_len(lens, shifts, nterms);
     if (ncomb) SA_TRY(get_workspace((void **)&pw, sizeof(fe) * ncomb, st, WS_COSET));
     DeviceTree b{st};
-    return coset_combine_evaluate(b, (fe *)out, log_n, root, offset, (const fe *const *)srcs, lens, shifts, weights,
-                                  nterms, pw);
+    return coset_combine_evaluate(b, (fe *)out, nrows, log_n, root, offset, (const fe *const *)srcs, lens, shifts,
+                                  rows, weights, nterms, pw);
+}
+
+int sa_coset_combine_evaluate(void *out, int log_n, const uint64_t root[2], const uint64_t offset[2],
+                              const void *const *srcs, const size_t *lens, const size_t *shifts,
+                              const uint64_t *weights, size_t nterms, void *stream) {
+    return sa_coset_combine_evaluate_batch(out, 1, log_n, root, offset, srcs, lens, shifts, nullptr, weights, nterms,
+                                           stream);
 }
 
 // ---- transition quotients (air.cuh) ----
@@ -612,29 +624,49 @@ int sa_air_plan(void *plan, const uint64_t *coeffs, const uint32_t *exps, const 
     return h ? SA_EDIVZERO : SA_OK;
 }
 
-// Reads the plan only; its scratch is the stream's workspace (WS_AIR): 2 nregs rows of n, and n per constraint of
-// a chunk
-int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
-                     size_t ncons, int log_n, const uint64_t root[2], void *stream) {
+size_t sa_air_batch_max(size_t nregs, size_t ncons, int log_n) { return air_batch_max(nregs, ncons, log_n); }
+
+// Reads the plan only; its scratch is the stream's workspace (WS_AIR): 2 nregs rows of n per trace of a chunk, and n
+// per constraint row of a row chunk (air_chunks)
+int sa_air_quotients_batch(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
+                           size_t ncons, size_t batch, int log_n, const uint64_t root[2], void *stream) {
     SA_TRY(air_apply_check(log_n, nregs, ncoef, qlen, ncons, root));
+    if (batch == 0) return SA_OK;
     cudaStream_t st = (cudaStream_t)stream;
+    const AirChunks k = air_chunks(nregs, ncons, batch, log_n);
     fe *ws = nullptr;
-    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, ncons, log_n), st, WS_AIR));
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, k, log_n), st, WS_AIR));
     DeviceAir b{{st}};
-    return air_quotients(b, (fe *)out, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons, log_n, root, ws);
+    return air_quotients(b, (fe *)out, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons, batch, log_n,
+                         root, ws, k);
 }
 
-// sa_air_quotients plus the flags: the same workspace, one memset and the exact store in place of k_coset_store
+int sa_air_quotients(void *out, const void *plan, const void *trace, size_t nregs, size_t ncoef, size_t qlen,
+                     size_t ncons, int log_n, const uint64_t root[2], void *stream) {
+    return sa_air_quotients_batch(out, plan, trace, nregs, ncoef, qlen, ncons, 1, log_n, root, stream);
+}
+
+// sa_air_quotients_batch plus the flags: the same workspace, one memset and the exact store in place of
+// k_coset_store
+int sa_air_quotients_exact_batch(void *out, uint32_t *flags, const void *plan, const void *trace, size_t nregs,
+                                 size_t ncoef, size_t qlen, size_t ncons, size_t batch, size_t tail, int log_n,
+                                 const uint64_t root[2], void *stream) {
+    SA_TRY(air_exact_check(log_n, nregs, ncoef, qlen, ncons, tail, root));
+    if (batch == 0) return SA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const AirChunks k = air_chunks(nregs, ncons, batch, log_n);
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, k, log_n), st, WS_AIR));
+    DeviceAirExact b{{{{st}}}};
+    return air_quotients_exact(b, (fe *)out, flags, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons,
+                               batch, tail, log_n, root, ws, k);
+}
+
 int sa_air_quotients_exact(void *out, uint32_t *flags, const void *plan, const void *trace, size_t nregs,
                            size_t ncoef, size_t qlen, size_t ncons, size_t tail, int log_n, const uint64_t root[2],
                            void *stream) {
-    SA_TRY(air_exact_check(log_n, nregs, ncoef, qlen, ncons, tail, root));
-    cudaStream_t st = (cudaStream_t)stream;
-    fe *ws = nullptr;
-    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * air_ws_elems(nregs, ncons, log_n), st, WS_AIR));
-    DeviceAirExact b{{{{st}}}};
-    return air_quotients_exact(b, (fe *)out, flags, (const fe *)plan, (const fe *)trace, nregs, ncoef, qlen, ncons,
-                               tail, log_n, root, ws);
+    return sa_air_quotients_exact_batch(out, flags, plan, trace, nregs, ncoef, qlen, ncons, 1, tail, log_n, root,
+                                        stream);
 }
 
 // ---- boundary quotients (boundary.cuh) ----

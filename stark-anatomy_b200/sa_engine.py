@@ -66,12 +66,19 @@ SYMBOLS = [
     ("sa_coset_batch_max", _sz, [_ci]),
     ("sa_coset_combine_evaluate", _ci, [_vp, _ci, _u64p, _u64p, ctypes.POINTER(ctypes.c_void_p),
                                         ctypes.POINTER(_sz), ctypes.POINTER(_sz), _u64p, _sz, _vp]),
+    ("sa_coset_combine_evaluate_batch", _ci, [_vp, _sz, _ci, _u64p, _u64p, ctypes.POINTER(ctypes.c_void_p),
+                                              ctypes.POINTER(_sz), ctypes.POINTER(_sz), ctypes.POINTER(_sz), _u64p,
+                                              _sz, _vp]),
     ("sa_air_plan_bytes", _sz, [_ci, _sz, _sz, _sz]),
     ("sa_air_plan", _ci, [_vp, _u64p, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(_sz), _sz, _sz, _sz, _vp, _sz,
                           _ci, _u64p, _u64p, _u64p, _vp]),
     ("sa_air_quotients", _ci, [_vp, _vp, _vp, _sz, _sz, _sz, _sz, _ci, _u64p, _vp]),
     ("sa_air_quotients_exact", _ci, [_vp, ctypes.POINTER(ctypes.c_uint32), _vp, _vp, _sz, _sz, _sz, _sz, _sz, _ci,
                                      _u64p, _vp]),
+    ("sa_air_quotients_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _sz, _sz, _sz, _ci, _u64p, _vp]),
+    ("sa_air_quotients_exact_batch", _ci, [_vp, ctypes.POINTER(ctypes.c_uint32), _vp, _vp, _sz, _sz, _sz, _sz, _sz,
+                                           _sz, _ci, _u64p, _vp]),
+    ("sa_air_batch_max", _sz, [_sz, _sz, _ci]),
     ("sa_boundary_plan_bytes", _sz, [_ci, _sz]),
     ("sa_boundary_plan", _ci, [_vp, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_sz),
                                ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_sz), _sz, _ci, _u64p, _u64p, _vp]),
@@ -82,6 +89,8 @@ SYMBOLS = [
     ("sa_merkle_tree_batch", _ci, [_vp, _vp, _sz, _sz, _vp]),
     ("sa_merkle_open_batch", _ci, [_vp, _vp, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_gather_batch", _ci, [_vp, _vp, _sz, _sz, _u64p, _sz, _vp]),
+    ("sa_merkle_open_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
+    ("sa_gather_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_commit", _ci, [_vp, _vp, _vp, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
@@ -470,6 +479,37 @@ class CudaEngine:
             self._stream()))
         return out
 
+    def coset_combine_evaluate_batch(self, terms, nrows, log_n, root, offset):
+        """sa_coset_combine_evaluate_batch: nrows combinations in one call -> (nrows, n, 2), row r the codeword
+        coset_combine_evaluate gives for the terms (vec, shift, weight, row) with row == r (zeros for a row without
+        terms), each vec a contiguous int64 (len, 2) tensor on this device; asynchronous, nothing is uploaded"""
+        torch = self.torch
+        nrows = int(nrows)
+        if self.lib.sa_coset_batch_max(log_n) == 0 or nrows < 0:
+            raise SaError(SA_ERRORS[-6])
+        n = 1 << log_n
+        ptrs, lens, shifts, rows, weights = [], [], [], [], []
+        for vec, shift, weight, row in terms:  # the library cannot see the tensors' shape, device or layout
+            if (not isinstance(vec, torch.Tensor) or vec.dtype != torch.int64 or vec.dim() != 2 or vec.shape[1] != 2
+                    or vec.device != self.device or not vec.is_contiguous()):
+                raise SaError(SA_ERRORS[-6])
+            shift, row = int(shift), int(row)
+            if shift < 0 or shift + vec.shape[0] > n or not 0 <= row < nrows:
+                raise SaError(SA_ERRORS[-6])
+            weight = int(weight) % P
+            ptrs.append(vec.data_ptr())
+            lens.append(vec.shape[0])
+            shifts.append(shift)
+            rows.append(row)
+            weights += [weight & 0xFFFFFFFFFFFFFFFF, weight >> 64]
+        t = len(ptrs)
+        out = torch.empty((nrows, n, 2), dtype=torch.int64, device=self.device)
+        self._check(self.lib.sa_coset_combine_evaluate_batch(
+            out.data_ptr(), nrows, log_n, _limbs(root), _limbs(offset), (ctypes.c_void_p * t)(*ptrs),
+            (ctypes.c_size_t * t)(*lens), (ctypes.c_size_t * t)(*shifts), (ctypes.c_size_t * t)(*rows),
+            (ctypes.c_uint64 * (2 * t))(*weights), t, self._stream()))
+        return out
+
     def air_plan(self, constraints, nregs, zerofier, max_ncoef, log_n, root, offset, step):
         """sa_air_plan: the transition constraints (MPolynomials or {exponent tuple: value} dicts over x, the nregs
         trace rows and the nregs next rows T(step * x)) compiled with the zerofier's (zlen, 2) coset division plan on
@@ -497,45 +537,56 @@ class CudaEngine:
             self._stream()))
         return AirPlan(plan, log_n, int(root), int(offset), nregs, ncons, max_ncoef, zerofier.shape[0] - 1)
 
-    def air_quotients(self, plan, trace, qlen):
-        """sa_air_quotients: the first qlen coefficients of every constraint's quotient for the trace polynomials
-        (nregs, ncoef, 2), ncoef <= the plan's max_ncoef -> (ncons, qlen, 2), in one call; asynchronous, the plan is
-        only read"""
+    def _air_trace(self, plan, trace, qlen):
+        """the batch of a (nregs, ncoef, 2) trace (None) or of a (B, nregs, ncoef, 2) batch of traces; "unsupported
+        size" otherwise (the library cannot see the tensor's shape, dtype or device)"""
         torch = self.torch
-        # the library cannot see the tensor's shape, dtype or device
         if (not isinstance(trace, torch.Tensor) or trace.dtype != torch.int64 or trace.device != self.device
-                or trace.dim() != 3 or trace.shape[0] != plan.nregs or trace.shape[2] != 2
-                or not 1 <= trace.shape[1] <= plan.max_ncoef or not 1 <= int(qlen) <= 1 << plan.log_n):
+                or trace.dim() not in (3, 4) or trace.shape[-3] != plan.nregs or trace.shape[-1] != 2
+                or not 1 <= trace.shape[-2] <= plan.max_ncoef or not 1 <= int(qlen) <= 1 << plan.log_n):
             raise SaError(SA_ERRORS[-6])
+        return trace.shape[0] if trace.dim() == 4 else None
+
+    def air_quotients(self, plan, trace, qlen):
+        """sa_air_quotients_batch: the first qlen coefficients of every constraint's quotient for the trace
+        polynomials (nregs, ncoef, 2), ncoef <= the plan's max_ncoef -> (ncons, qlen, 2), or for a batch of traces
+        (B, nregs, ncoef, 2) -> (B, ncons, qlen, 2), in one call; asynchronous, the plan is only read"""
+        torch = self.torch
+        batch = self._air_trace(plan, trace, qlen)
         trace = trace.contiguous()
-        out = torch.empty((plan.ncons, int(qlen), 2), dtype=torch.int64, device=self.device)
-        self._check(self.lib.sa_air_quotients(out.data_ptr(), plan.plan.data_ptr(), trace.data_ptr(), plan.nregs,
-                                              trace.shape[1], int(qlen), plan.ncons, plan.log_n, _limbs(plan.root),
-                                              self._stream()))
+        out = torch.empty(tuple(trace.shape[:-3]) + (plan.ncons, int(qlen), 2), dtype=torch.int64, device=self.device)
+        self._check(self.lib.sa_air_quotients_batch(out.data_ptr(), plan.plan.data_ptr(), trace.data_ptr(),
+                                                    plan.nregs, trace.shape[-2], int(qlen), plan.ncons,
+                                                    1 if batch is None else batch, plan.log_n, _limbs(plan.root),
+                                                    self._stream()))
         return out
 
     def air_quotients_exact(self, plan, trace, qlen, check=True):
-        """sa_air_quotients_exact: air_quotients' rows (ncons, qlen, 2) and the remainder flags (ncons,) int32,
+        """sa_air_quotients_exact_batch: air_quotients' rows (ncons, qlen, 2) and the remainder flags (ncons,) int32,
         non-zero exactly where Z does not divide the constraint's numerator (the reference's Polynomial.__truediv__
-        test), with the tail n - deg Z.  The zerofier's top coefficient must be non-zero (deg Z = its length - 1, as
-        air_plan takes it).  check=True reads the flags (one synchronisation) and raises the reference's remainder
-        message naming the constraints; check=False stays asynchronous.  The plan is only read."""
+        test), with the tail n - deg Z; for a batch of traces (B, nregs, ncoef, 2) the rows (B, ncons, qlen, 2) and
+        flags (B, ncons).  The zerofier's top coefficient must be non-zero (deg Z = its length - 1, as air_plan takes
+        it).  check=True reads the flags (one synchronisation) and raises the reference's remainder message naming the
+        constraints (for a batch, the (trace, constraint) pairs); check=False stays asynchronous.  The plan is only
+        read."""
         torch = self.torch
-        if (not isinstance(trace, torch.Tensor) or trace.dtype != torch.int64 or trace.device != self.device
-                or trace.dim() != 3 or trace.shape[0] != plan.nregs or trace.shape[2] != 2
-                or not 1 <= trace.shape[1] <= plan.max_ncoef or not 1 <= int(qlen) <= 1 << plan.log_n
-                or plan.zdeg is None):
+        batch = self._air_trace(plan, trace, qlen)
+        if plan.zdeg is None:
             raise SaError(SA_ERRORS[-6])
         trace = trace.contiguous()
-        out = torch.empty((plan.ncons, int(qlen), 2), dtype=torch.int64, device=self.device)
-        flags = torch.empty(plan.ncons, dtype=torch.int32, device=self.device)
-        self._check(self.lib.sa_air_quotients_exact(
+        lead = tuple(trace.shape[:-3])
+        out = torch.empty(lead + (plan.ncons, int(qlen), 2), dtype=torch.int64, device=self.device)
+        flags = torch.empty(lead + (plan.ncons,), dtype=torch.int32, device=self.device)
+        self._check(self.lib.sa_air_quotients_exact_batch(
             out.data_ptr(), ctypes.cast(flags.data_ptr(), ctypes.POINTER(ctypes.c_uint32)), plan.plan.data_ptr(),
-            trace.data_ptr(), plan.nregs, trace.shape[1], int(qlen), plan.ncons, (1 << plan.log_n) - plan.zdeg,
-            plan.log_n, _limbs(plan.root), self._stream()))
+            trace.data_ptr(), plan.nregs, trace.shape[-2], int(qlen), plan.ncons, 1 if batch is None else batch,
+            (1 << plan.log_n) - plan.zdeg, plan.log_n, _limbs(plan.root), self._stream()))
         if check:
-            self._count("d2h", 4 * plan.ncons)
-            bad = [c for c, f in enumerate(flags.tolist()) if f]
+            self._count("d2h", 4 * flags.numel())
+            if batch is None:
+                bad = [c for c, f in enumerate(flags.tolist()) if f]
+            else:
+                bad = [(b, c) for b, row in enumerate(flags.tolist()) for c, f in enumerate(row) if f]
             if bad:
                 raise SaError("%s (constraints %s)" % (REMAINDER, bad))
         return out, flags
@@ -680,41 +731,64 @@ class CudaEngine:
         raw = trees[:, 1].cpu().numpy().tobytes()
         return [raw[64 * b:64 * (b + 1)] for b in range(trees.shape[0])]
 
-    def merkle_open_batch(self, trees, indices):
-        """sa_merkle_open_batch: for each tree of a (B, 2n, 64) batch, the authentication paths of the same leaf
-        indices (B lists of k lists of 64-byte digests, bottom-up), with one upload and one download"""
+    @staticmethod
+    def _index_sets(batch, n, indices, group):
+        """(the group, k, the flat index list) of a call's index sets: one set `indices` when group is None, else
+        indices is a list of ceil(batch / group) sets of one length k, set g for rows g * group .. g * group + group;
+        "unsupported size" or "cannot open invalid index" before any device work"""
+        if group is None:
+            sets, group = [list(indices)], max(batch, 1)
+        else:
+            group, sets = int(group), [list(s) for s in indices]
+            if group < 1 or len(sets) != max(1, -(-batch // group)) or len({len(s) for s in sets}) > 1:
+                raise SaError(SA_ERRORS[-6])
+        flat = [i for s in sets for i in s]
+        for i in flat:
+            if not 0 <= i < n:
+                raise SaError(SA_ERRORS[-5])
+        return group, len(sets[0]), flat
+
+    def merkle_open_batch(self, trees, indices, group=None):
+        """sa_merkle_open_batch_sets: for each tree of a (B, 2n, 64) batch, the authentication paths of the same leaf
+        indices, or with `group`, of its group's own set indices[b // group] (B lists of k lists of 64-byte digests,
+        bottom-up), with one upload and one download"""
         if trees.dim() != 3 or trees.shape[1] < 2 or trees.shape[1] % 2 or trees.shape[2] != 64:
             raise SaError(SA_ERRORS[-6])
         trees = trees.contiguous()
-        batch, n, k = trees.shape[0], trees.shape[1] // 2, len(indices)
+        batch, n = trees.shape[0], trees.shape[1] // 2
+        group, k, flat = self._index_sets(batch, n, indices, group)
         depth = n.bit_length() - 1
-        for i in indices:
-            if not 0 <= i < n:
-                raise SaError(SA_ERRORS[-5])
         out = self.torch.empty((batch, k, depth, 64), dtype=self.torch.uint8, device=self.device)
-        idx = (ctypes.c_uint64 * k)(*indices)
-        self._check(self.lib.sa_merkle_open_batch(out.data_ptr(), trees.data_ptr(), n, batch, idx, k, self._stream()))
+        idx = (ctypes.c_uint64 * max(len(flat), 1))(*flat)
+        self._check(self.lib.sa_merkle_open_batch_sets(out.data_ptr(), trees.data_ptr(), n, batch, group, idx, k,
+                                                       self._stream()))
         if out.numel() == 0:  # no tree, no index or no sibling: nothing was launched
-            return [[[] for _ in indices] for _ in range(batch)]
-        self._count("h2d", 8 * k)
+            return [[[] for _ in range(k)] for _ in range(batch)]
+        self._count("h2d", 8 * len(flat))
         self._count("d2h", out.numel())
         raw = out.cpu().numpy().tobytes()
         digests = [raw[i:i + 64] for i in range(0, len(raw), 64)]
         paths = [digests[i:i + depth] for i in range(0, len(digests), depth)]
         return [paths[b * k:(b + 1) * k] for b in range(batch)]
 
-    def gather_batch(self, vecs, indices):
-        """sa_gather_batch: the values at the same indices in each row of a (B, n, 2) batch -> numpy (B, k, 2) on
-        the host (the int64 limbs `gather` returns), with one upload and one download"""
+    def gather_batch(self, vecs, indices, group=None):
+        """sa_gather_batch_sets: the values at the same indices in each row of a (B, n, 2) batch, or with `group`, at
+        the row's group's own set indices[b // group] -> numpy (B, k, 2) on the host (the int64 limbs `gather`
+        returns), with one upload and one download"""
         if vecs.dim() != 3 or vecs.shape[-1] != 2:
             raise SaError(SA_ERRORS[-6])
         vecs = vecs.contiguous()
-        batch, n, k = vecs.shape[0], vecs.shape[1], len(indices)
+        batch, n = vecs.shape[0], vecs.shape[1]
+        if group is None:  # the library checks a lone set's indices itself
+            group, k, flat = max(batch, 1), len(indices), list(indices)
+        else:
+            group, k, flat = self._index_sets(batch, n, indices, group)
         out = self.torch.empty((batch, k, 2), dtype=self.torch.int64, device=self.device)
-        idx = (ctypes.c_uint64 * k)(*indices)
-        self._check(self.lib.sa_gather_batch(out.data_ptr(), vecs.data_ptr(), n, batch, idx, k, self._stream()))
+        idx = (ctypes.c_uint64 * max(len(flat), 1))(*flat)
+        self._check(self.lib.sa_gather_batch_sets(out.data_ptr(), vecs.data_ptr(), n, batch, group, idx, k,
+                                                  self._stream()))
         if out.numel():
-            self._count("h2d", 8 * k)
+            self._count("h2d", 8 * len(flat))
             self._count("d2h", out.numel() * 8)
         return out.cpu().numpy()
 

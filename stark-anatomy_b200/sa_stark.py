@@ -27,6 +27,12 @@ RPSSS.sign): the stages above are shared code, the transition quotients come fro
 per-constraint flag is exactly the reference's exact-division test (DESIGN section 3.10), and there are no zerofier
 openings.
 
+``prove_batch`` proves many statements of one plan's AIR in one call: the stages before FRI run once for the whole
+batch (one interpolation, one boundary apply, one transition apply per division order, one commitment, one
+combination into one codeword per proof, one gather and one path read for all openings), FRI runs per proof, and each
+proof is the bytes ``prove`` gives from the same draws (DESIGN section 3.11); ``prove`` is ``prove_batch`` of one.
+``sign_batch`` signs many documents with one key on an RPSSS or FastRPSSS instance.
+
 ``enable(cls)`` rebinds ``cls.prove`` (FastStark's) to ``prove``, ``enable_plain(cls)`` rebinds Stark's to
 ``prove_plain``; ``disable()`` restores both.  Off by default, as ``sa_accel``.  Nothing here imports torch or holds
 device state outside a plan.
@@ -153,36 +159,83 @@ class _Stages:
         domain = [FieldElement(pow(omicron, i, P), stark.field) for i in range(self.trace_length)]
         self.interp = eng.interp_plan(eng.upload(sa_devlist.pack(domain)))
 
-    def _trace_polynomials(self, eng, trace):
-        """the trace randomizers, drawn in the reference's order (the caller's list is not touched), one upload of
-        the columns and one batched interpolation: the (nregs, T, 2) trace polynomials"""
+    def _trace_polynomials(self, eng, traces):
+        """every proof's trace randomizers, drawn proof by proof and row by row in the reference's order (the
+        callers' lists are not touched), one upload of all columns and one batched interpolation: the (B nregs, T, 2)
+        trace polynomials, proof b's register s in row b nregs + s"""
         stark, field, nregs, T = self.stark, self.stark.field, self.nregs, self.trace_length
-        assert len(trace) == self.ncycles, \
-            "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
-        rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
-                              for k in range(stark.num_randomizers)]
-        columns = eng.upload(sa_devlist.pack([rows[c][s] for s in range(nregs) for c in range(T)]))
-        return eng.interp_apply(self.interp, columns.reshape(nregs, T, 2))
+        for trace in traces:
+            assert len(trace) == self.ncycles, \
+                "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
+        values = []
+        for trace in traces:
+            rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
+                                  for k in range(stark.num_randomizers)]
+            values += [rows[c][s] for s in range(nregs) for c in range(T)]
+        columns = eng.upload(sa_devlist.pack(values))
+        return eng.interp_apply(self.interp, columns.reshape(len(traces) * nregs, T, 2))
 
-    def _boundary(self, eng, polys, boundary):
-        """(the (nregs + 1, n, 2) commitment buffer with the boundary codewords in its first rows, the boundary
-        quotients, their degree bounds); the reference's remainder message when a boundary value is false"""
-        stark, nregs, log_n = self.stark, self.nregs, self.log_n
-        bplan = eng.boundary_plan(boundary, nregs, stark.omicron, log_n, stark.omega.value, stark.generator.value)
-        committed = eng.empty((nregs + 1) << log_n).reshape(nregs + 1, 1 << log_n, 2)
-        bquot, _, _ = eng.boundary_quotients(bplan, polys, check=True, out=committed[:nregs])
-        return committed, bquot, bplan.degree_bounds(self.trace_length)
+    def _boundary(self, eng, polys, boundaries, failed):
+        """(the (B, nregs + 1, n, 2) commitment buffer with each proof's boundary codewords in its first rows, the
+        boundary quotients, each proof's degree bounds) from one boundary plan of B nregs registers, register
+        b nregs + s being proof b's register s; a proof whose boundary value is false gets the reference's remainder
+        message in `failed`.  None when the plan of all boundaries is refused (``_refused`` finds the proof)."""
+        stark, nregs, log_n, B = self.stark, self.nregs, self.log_n, len(boundaries)
+        n = 1 << log_n
+        merged = [(c, b * nregs + int(r), v) for b, boundary in enumerate(boundaries) for c, r, v in boundary]
+        try:
+            bplan = eng.boundary_plan(merged, B * nregs, stark.omicron, log_n, stark.omega.value,
+                                      stark.generator.value)
+        except AssertionError:
+            return None
+        committed = eng.empty(B * (nregs + 1) << log_n).reshape(B, nregs + 1, n, 2)
+        # a proof's rows are contiguous in the buffer, so a batch of one writes its codewords there directly
+        bquot, bcw, flags = eng.boundary_quotients(bplan, polys, check=False,
+                                                   out=committed[0, :nregs] if B == 1 else None)
+        if B > 1:
+            committed[:, :nregs] = bcw.reshape(B, nregs, n, 2)
+        flags = flags.tolist()
+        for b in range(B):
+            bad = [s for s in range(nregs) if flags[b * nregs + s]]
+            if bad:
+                failed.setdefault(b, sa_engine.SaError("%s (registers %s)" % (REMAINDER, bad)))
+        bounds = bplan.degree_bounds(self.trace_length)
+        return committed, bquot, [bounds[b * nregs:(b + 1) * nregs] for b in range(B)]
 
-    def _commit(self, eng, committed, proof_stream):
-        """the randomizer polynomial, drawn where the reference draws it, its codeword in the buffer's last row, one
-        commitment of every row and their roots pushed in order: (the randomizer, the trees)"""
-        stark, nregs, log_n = self.stark, self.nregs, self.log_n
-        randomizer = [stark.field.sample(os.urandom(17)) for i in range(self.max_degree + 1)]
-        rvec = eng.upload(sa_devlist.pack(randomizer))
-        eng.coset_evaluate(rvec, log_n, stark.omega.value, stark.generator.value, out=committed[nregs])
-        trees = eng.merkle_trees(committed)
-        for root in eng.tree_roots(trees):
-            proof_stream.push(root)
+    def _refused(self, eng, boundaries):
+        """the lowest proof whose own boundary plan is refused, and its exception"""
+        stark = self.stark
+        for b, boundary in enumerate(boundaries):
+            try:
+                eng.boundary_plan(boundary, self.nregs, stark.omicron, self.log_n, stark.omega.value,
+                                  stark.generator.value)
+            except AssertionError as e:
+                return b, e
+        raise AssertionError("sa_stark: the boundary plan of the batch was refused, and no proof's own")
+
+    def _randomizers(self, count):
+        """the randomizer polynomials of the first `count` proofs, drawn proof by proof where the reference draws
+        each proof's"""
+        field = self.stark.field
+        return [[field.sample(os.urandom(17)) for i in range(self.max_degree + 1)] for b in range(count)]
+
+    def _commit(self, eng, committed, randomizers, proof_streams):
+        """every proof's randomizer codeword in its last row of the buffer (one batched coset_evaluate), one
+        commitment of all B (nregs + 1) rows, and each proof's roots pushed in order into its stream: (the (B,
+        max_degree + 1, 2) randomizers, the trees)"""
+        stark, nregs, log_n, B = self.stark, self.nregs, self.log_n, len(randomizers)
+        rvec = eng.upload(sa_devlist.pack([r for rs in randomizers for r in rs]))
+        if B == 1:
+            eng.coset_evaluate(rvec, log_n, stark.omega.value, stark.generator.value, out=committed[0, nregs])
+            rvec = rvec.reshape(1, self.max_degree + 1, 2)
+        else:
+            rvec = rvec.reshape(B, self.max_degree + 1, 2)
+            committed[:, nregs] = eng.coset_evaluate(rvec, log_n, stark.omega.value, stark.generator.value)
+        trees = eng.merkle_trees(committed.reshape(B * (nregs + 1), 1 << log_n, 2))
+        roots = eng.tree_roots(trees)
+        for b, ps in enumerate(proof_streams):
+            for root in roots[b * (nregs + 1):(b + 1) * (nregs + 1)]:
+                ps.push(root)
         return rvec, trees
 
     def _weights(self, proof_stream):
@@ -190,38 +243,98 @@ class _Stages:
         number = 1 + 2 * len(self.constraints) + 2 * self.nregs
         return [w.value for w in self.stark.sample_weights(number, proof_stream.prover_fiat_shamir())]
 
-    def _combine_prove_open(self, eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_stream):
-        """the combination of the randomizer, each transition quotient row (rows: (the row truncated to its bound
-        + 1, the bound)) and each boundary quotient at shift 0 and at max_degree - bound; FRI on its codeword; the
-        openings of the committed codewords.  An empty row (a zero quotient) adds nothing and is left out.
-        Returns the quadrupled indices."""
-        stark, field, nregs, log_n = self.stark, self.stark.field, self.nregs, self.log_n
+    def _combine_prove_open(self, eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_streams):
+        """for each proof b the combination of its randomizer, each transition quotient row (rows[b]: (the row
+        truncated to its bound + 1, the bound)) and each boundary quotient at shift 0 and at max_degree - bound, all
+        B codewords from one call; FRI on each proof's codeword, proof by proof; then one gather and one path read
+        of every proof's committed codewords at that proof's own indices.  An empty row (a zero quotient) adds
+        nothing and is left out.  Returns each proof's quadrupled indices."""
+        stark, field, nregs, log_n, B = self.stark, self.stark.field, self.nregs, self.log_n, len(proof_streams)
         n = 1 << log_n
-        terms = [(rvec, 0, weights[0])]
-        for c, (q, bound) in enumerate(rows):
-            if bound >= 0:
-                terms += [(q, 0, weights[1 + 2 * c]), (q, self.max_degree - bound, weights[2 + 2 * c])]
-        base = 1 + 2 * len(rows)
-        for s, bound in enumerate(bounds_b):
-            q = bquot[s, :bound + 1]
-            terms += [(q, 0, weights[base + 2 * s]), (q, self.max_degree - bound, weights[base + 2 * s + 1])]
-        combined = eng.coset_combine_evaluate(terms, log_n, stark.omega.value, stark.generator.value)
+        terms = []
+        for b in range(B):
+            w = weights[b]
+            terms.append((rvec[b], 0, w[0], b))
+            for c, (q, bound) in enumerate(rows[b]):
+                if bound >= 0:
+                    terms += [(q, 0, w[1 + 2 * c], b), (q, self.max_degree - bound, w[2 + 2 * c], b)]
+            base = 1 + 2 * len(rows[b])
+            for s, bound in enumerate(bounds_b[b]):
+                q = bquot[b * nregs + s, :bound + 1]
+                terms += [(q, 0, w[base + 2 * s], b), (q, self.max_degree - bound, w[base + 2 * s + 1], b)]
+        args = (log_n, stark.omega.value, stark.generator.value)
+        # a batch of one is the single-codeword call: nrows = 1 of the same kernel
+        if B == 1:
+            combined = eng.coset_combine_evaluate([t[:3] for t in terms], *args).reshape(1, n, 2)
+        else:
+            combined = eng.coset_combine_evaluate_batch(terms, B, *args)
 
-        indices = self.fri.prove(sa_devlist.DeviceCodeword(combined, None, field, n), proof_stream)
-
-        duplicated = list(indices) + [(i + stark.expansion_factor) % n for i in indices]
-        quadrupled = duplicated + [(i + n // 2) % n for i in duplicated]
-        quadrupled.sort()
-        distinct = sorted(set(quadrupled))
-        raw = eng.gather_batch(committed, distinct)
-        paths = eng.merkle_open_batch(trees, quadrupled)
-        for b in range(nregs + 1):
-            # a repeated index pushes the same element object, as indexing one list does; every path is its own
-            values = dict(zip(distinct, sa_marshal.unpack(raw[b], field, FieldElement)))
-            for q, i in enumerate(quadrupled):
-                proof_stream.push(values[i])
-                proof_stream.push(paths[b][q])
+        quadrupled = []
+        for b, ps in enumerate(proof_streams):
+            indices = self.fri.prove(sa_devlist.DeviceCodeword(combined[b], None, field, n), ps)
+            duplicated = list(indices) + [(i + stark.expansion_factor) % n for i in indices]
+            quadrupled.append(sorted(duplicated + [(i + n // 2) % n for i in duplicated]))
+        # each proof's distinct indices, padded with its last one to a common length
+        distinct = [sorted(set(q)) for q in quadrupled]
+        width = max(len(d) for d in distinct)
+        distinct = [d + d[-1:] * (width - len(d)) for d in distinct]
+        rows2d = committed.reshape(B * (nregs + 1), n, 2)
+        if B == 1:
+            raw = eng.gather_batch(rows2d, distinct[0])
+            paths = eng.merkle_open_batch(trees, quadrupled[0])
+        else:
+            raw = eng.gather_batch(rows2d, distinct, group=nregs + 1)
+            paths = eng.merkle_open_batch(trees, quadrupled, group=nregs + 1)
+        for b, ps in enumerate(proof_streams):
+            for r in range(b * (nregs + 1), (b + 1) * (nregs + 1)):
+                # a repeated index pushes the same element object, as indexing one list does; every path is its own
+                values = dict(zip(distinct[b], sa_marshal.unpack(raw[r], field, FieldElement)))
+                for q, i in enumerate(quadrupled[b]):
+                    ps.push(values[i])
+                    ps.push(paths[r][q])
         return quadrupled
+
+    def _prove_batch(self, traces, boundaries, proof_streams, transition):
+        """the schedule both provers share: (the proof streams, each proof's quadrupled indices).  transition(eng,
+        polys, failed, B) runs the plan's transition quotients and their checks for every proof not yet in `failed`
+        and returns (rows_of, degree_check): rows_of(b) gives proof b's combination rows, degree_check(eng, live,
+        failed) checks the proofs below `live`."""
+        eng = sa_engine.get_engine()
+        B = len(traces)
+        assert len(boundaries) == B, "sa_stark: %d traces and %d boundaries" % (B, len(boundaries))
+        if proof_streams is None:
+            proof_streams = [sa_host.ip.ProofStream() for b in range(B)]
+        assert len(proof_streams) == B, "sa_stark: %d traces and %d proof streams" % (B, len(proof_streams))
+        if B == 0:
+            return [], []
+
+        polys = self._trace_polynomials(eng, traces)
+        failed = {}  # proof -> the exception proving it alone raises first
+        stage = self._boundary(eng, polys, boundaries, failed)
+        if stage is None:
+            # a boundary the plan refuses: the proofs before the lowest such proof run as a batch of their own
+            b, exc = self._refused(eng, boundaries)
+            self._prove_batch(traces[:b], boundaries[:b], proof_streams[:b], transition)
+            exc.proof_index = b
+            raise exc
+        committed, bquot, bounds_b = stage
+        rows_of, degree_check = transition(eng, polys, failed, B)
+
+        # the proofs before the lowest failed one go on: their randomizers, and their degree checks
+        live = min(failed) if failed else B
+        randomizers = self._randomizers(live)
+        if not failed:
+            rvec, trees = self._commit(eng, committed, randomizers, proof_streams)
+            weights = [self._weights(ps) for ps in proof_streams]
+        degree_check(eng, live, failed)
+        if failed:
+            b = min(failed)
+            failed[b].proof_index = b
+            raise failed[b]
+
+        quadrupled = self._combine_prove_open(eng, rvec, [rows_of(b) for b in range(B)], bquot, bounds_b, weights,
+                                              committed, trees, proof_streams)
+        return proof_streams, quadrupled
 
 
 class StarkPlan(_Stages):
@@ -313,67 +426,80 @@ class StarkPlan(_Stages):
 
     def prove(self, trace, boundary, transition_zerofier_codeword, proof_stream=None):
         """FastStark.prove(trace, constraints, boundary, zerofier, zerofier_codeword, proof_stream) for this plan's
-        constraints and zerofier: proof_stream.serialize()"""
-        eng = sa_engine.get_engine()
-        T = self.trace_length
-        if proof_stream is None:
-            proof_stream = sa_host.ip.ProofStream()
+        constraints and zerofier: proof_stream.serialize().  It is prove_batch of one."""
+        return self.prove_batch([trace], [boundary], transition_zerofier_codeword,
+                                None if proof_stream is None else [proof_stream])[0]
 
-        # trace randomizers and trace polynomials (:82-90), boundary quotients (:93-106)
-        polys = self._trace_polynomials(eng, trace)
-        committed, bquot, bounds_b = self._boundary(eng, polys, boundary)
-
-        # transition quotients (:108-113), each constraint at the order the reference divides it at
-        tops = [_value(lo, hi) for lo, hi in eng.gather_batch(polys, [T - 1]).reshape(self.nregs, 2).tolist()]
-        quots = [eng.air_quotients(plan, polys, qlen) for _, plan, _, qlen in self.groups]
+    def prove_batch(self, traces, boundaries, transition_zerofier_codeword, proof_streams=None):
+        """FastStark.prove for each (traces[b], boundaries[b], proof_streams[b]) with this plan's constraints and
+        zerofier, the pre-FRI stages of all proofs in one schedule: the list of proof bytes, proof b's the bytes
+        proving it alone gives from the same draws (DESIGN section 3.11 gives the draw order).  The exception is the
+        one proving the proofs one at a time in order raises first, with the failing proof's index as
+        ``proof_index``."""
+        T, nregs = self.trace_length, self.nregs
         where = self._where()
-        long_rows = {}
-        for k in self.cons:
-            # a non-zero top coefficient makes the numerator's degree k.degree, so the reference's order is k.order
-            assert self._top_coefficient(k, tops), "sa_stark: the numerator of transition constraint %d is below " \
-                "its degree bound %d; its division order cannot be decided exactly" % (k.index, k.degree)
-            assert k.kind != "larger", LARGER_DEGREE
-            if k.kind == "long":
-                g, j = where[k.index]
-                if g not in long_rows:
-                    long_rows[g] = sa_marshal.unpack(eng.download(quots[g].reshape(-1, 2)), self.stark.field,
-                                                     FieldElement)
-                qlen = self.groups[g][3]
-                tail = long_rows[g][j * qlen + k.bound + 1:(j + 1) * qlen]
-                assert not any(v.value for v in tail), REMAINDER
 
-        # randomizer polynomial and the commitment (:116-119), weights (:125)
-        rvec, trees = self._commit(eng, committed, proof_stream)
-        weights = self._weights(proof_stream)
+        def transition(eng, polys, failed, B):
+            # transition quotients (:108-113), each constraint at the order the reference divides it at
+            tops = [_value(lo, hi) for lo, hi in eng.gather_batch(polys, [T - 1]).reshape(B * nregs, 2).tolist()]
+            batched = polys if B == 1 else polys.reshape(B, nregs, T, 2)
+            quots = [eng.air_quotients(plan, batched, qlen) for _, plan, _, qlen in self.groups]
+            quots = [q.reshape((B,) + tuple(q.shape[-3:])) for q in quots]
+            long_rows = {}
+            for b in range(B):
+                for k in self.cons:
+                    if b in failed:
+                        break
+                    # a non-zero top coefficient makes the numerator's degree k.degree, so the reference's order is
+                    # k.order
+                    if not self._top_coefficient(k, tops[b * nregs:(b + 1) * nregs]):
+                        failed[b] = AssertionError("sa_stark: the numerator of transition constraint %d is below its "
+                                                   "degree bound %d; its division order cannot be decided exactly"
+                                                   % (k.index, k.degree))
+                    elif k.kind == "larger":
+                        failed[b] = AssertionError(LARGER_DEGREE)
+                    elif k.kind == "long":
+                        g, j = where[k.index]
+                        if g not in long_rows:  # one download of the group's rows for every proof
+                            long_rows[g] = sa_marshal.unpack(eng.download(quots[g].reshape(-1, 2)), self.stark.field,
+                                                             FieldElement)
+                        qlen, ng = self.groups[g][3], len(self.groups[g][2])
+                        at = (b * ng + j) * qlen
+                        if any(v.value for v in long_rows[g][at + k.bound + 1:at + qlen]):
+                            failed[b] = AssertionError(REMAINDER)
 
-        # the degree check (:127): each quotient's coefficient at its bound is non-zero
-        for g, (_, _, idx, qlen) in enumerate(self.groups):
-            if self.cons[idx[0]].kind == "transform":
-                at = [j * qlen + self.cons[c].bound for j, c in enumerate(idx)]
-                vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
-                assert all(int(lo) or int(hi) for lo, hi in vals), DEGREE_MISMATCH
+            def degree_check(eng, live, failed):
+                # the degree check (:127): each quotient's coefficient at its bound is non-zero
+                for g, (_, _, idx, qlen) in enumerate(self.groups):
+                    if self.cons[idx[0]].kind == "transform" and live:
+                        at = [(b * len(idx) + j) * qlen + self.cons[c].bound for b in range(live)
+                              for j, c in enumerate(idx)]
+                        vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
+                        for b in range(live):
+                            chunk = vals[b * len(idx):(b + 1) * len(idx)]
+                            if not all(int(lo) or int(hi) for lo, hi in chunk):
+                                failed.setdefault(b, AssertionError(DEGREE_MISMATCH))
 
-        # the combination (:129-148), FRI (:151) and the boundary and randomizer openings (:154-169)
-        rows = []
-        for k in self.cons:
-            g, j = where[k.index]
-            rows.append((quots[g][j, :k.bound + 1], k.bound))
-        quadrupled = self._combine_prove_open(eng, rvec, rows, bquot, bounds_b, weights, committed, trees,
-                                              proof_stream)
+            def rows_of(b):
+                return [(quots[where[k.index][0]][b, where[k.index][1], :k.bound + 1], k.bound) for k in self.cons]
+            return rows_of, degree_check
 
-        # ... and the zerofier's (:171-175)
+        streams, quadrupled = self._prove_batch(list(traces), list(boundaries), proof_streams, transition)
+
+        # ... and the zerofier's openings (:171-175), proof by proof: the codeword is the caller's
         zc = transition_zerofier_codeword
-        if isinstance(zc, sa_devlist.DeviceCodeword):
-            zc.prefetch(quadrupled)
-            zpaths = zc.open_paths(quadrupled)
-        else:
-            tree = _fri.Merkle._device_tree(zc)
-            zpaths = ([_fri.Merkle.open(i, zc) for i in quadrupled] if tree is None or len(zc) < 2
-                      else eng.merkle_open(tree, quadrupled))
-        for q, i in enumerate(quadrupled):
-            proof_stream.push(zc[i])
-            proof_stream.push(zpaths[q])
-        return proof_stream.serialize()
+        for ps, quad in zip(streams, quadrupled):
+            if isinstance(zc, sa_devlist.DeviceCodeword):
+                zc.prefetch(quad)
+                zpaths = zc.open_paths(quad)
+            else:
+                tree = _fri.Merkle._device_tree(zc)
+                zpaths = ([_fri.Merkle.open(i, zc) for i in quad] if tree is None or len(zc) < 2
+                          else sa_engine.get_engine().merkle_open(tree, quad))
+            for q, i in enumerate(quad):
+                ps.push(zc[i])
+                ps.push(zpaths[q])
+        return [ps.serialize() for ps in streams]
 
 
 def prove(stark, trace, transition_constraints, boundary, transition_zerofier, transition_zerofier_codeword,
@@ -442,47 +568,93 @@ class PlainStarkPlan(_Stages):
 
     def prove(self, trace, boundary, proof_stream=None):
         """Stark.prove(trace, constraints, boundary, proof_stream) for this plan's constraints:
-        proof_stream.serialize()"""
-        eng = sa_engine.get_engine()
-        if proof_stream is None:
-            proof_stream = sa_host.ip.ProofStream()
+        proof_stream.serialize().  It is prove_batch of one."""
+        return self.prove_batch([trace], [boundary], None if proof_stream is None else [proof_stream])[0]
 
-        # trace randomizers and trace polynomials (stark.py:79-87), boundary quotients (:90-104)
-        polys = self._trace_polynomials(eng, trace)
-        committed, bquot, bounds_b = self._boundary(eng, polys, boundary)
+    def prove_batch(self, traces, boundaries, proof_streams=None):
+        """Stark.prove for each (traces[b], boundaries[b], proof_streams[b]) with this plan's constraints, the
+        pre-FRI stages of all proofs in one schedule: the list of proof bytes, proof b's the bytes proving it alone
+        gives from the same draws (DESIGN section 3.11).  The exception is the one proving the proofs one at a time
+        in order raises first, with the failing proof's index as ``proof_index``."""
+        T, nregs = self.trace_length, self.nregs
 
-        # transition quotients (:107-111): exact divisions, the remainder message before the randomizer is drawn
-        if not self.groups:
-            raise IndexError("list index out of range")  # zerofier_domain of no points (univariate.py:123)
-        quots = [eng.air_quotients_exact(plan, polys, qlen, check=True)[0] for plan, _, qlen in self.groups]
+        def transition(eng, polys, failed, B):
+            # transition quotients (stark.py:107-111): exact divisions, the remainder message before the randomizer
+            # is drawn
+            if not self.groups:  # zerofier_domain of no points (univariate.py:123)
+                for b in range(B):
+                    failed.setdefault(b, IndexError("list index out of range"))
+                return None, lambda eng, live, failed: None
+            batched = polys if B == 1 else polys.reshape(B, nregs, T, 2)
+            quots, flags = [], []
+            for plan, _, qlen in self.groups:
+                q, f = eng.air_quotients_exact(plan, batched, qlen, check=False)
+                quots.append(q.reshape((B,) + tuple(q.shape[-3:])))
+                flags.append(f.reshape(B, -1).tolist())
+            for b in range(B):
+                for f in flags:
+                    bad = [j for j, x in enumerate(f[b]) if x]
+                    if bad:
+                        failed.setdefault(b, sa_engine.SaError("%s (constraints %s)" % (REMAINDER, bad)))
+                        break
 
-        # randomizer polynomial and the commitment (:114-117), weights (:123)
-        rvec, trees = self._commit(eng, committed, proof_stream)
-        weights = self._weights(proof_stream)
+            def degree_check(eng, live, failed):
+                # the degree check (:125).  A clean row U_c vanishes above deg N_c - deg Z <= b_c, so the quotient
+                # has degree b_c exactly when U_c[b_c] != 0.  For b_c < 0, deg N_c <= D_c < deg Z and Z | N_c force
+                # N_c = 0: the quotient is Polynomial([]), of degree -1 (univariate.py:8-9, 83-84), which matches
+                # b_c = -1 only.
+                ok = [all(c >= -1 for c in self.bounds)] * live
+                for g, (_, idx, qlen) in enumerate(self.groups):
+                    js = [j for j, c in enumerate(idx) if self.bounds[c] >= 0]
+                    if js and live:
+                        at = [(b * len(idx) + j) * qlen + self.bounds[idx[j]] for b in range(live) for j in js]
+                        vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
+                        for b in range(live):
+                            ok[b] = ok[b] and all(int(lo) or int(hi) for lo, hi in vals[b * len(js):(b + 1) * len(js)])
+                for b in range(live):
+                    if not ok[b]:
+                        failed.setdefault(b, AssertionError(DEGREE_MISMATCH))
 
-        # the degree check (:125).  A clean row U_c vanishes above deg N_c - deg Z <= b_c, so the quotient has
-        # degree b_c exactly when U_c[b_c] != 0.  For b_c < 0, deg N_c <= D_c < deg Z and Z | N_c force N_c = 0: the
-        # quotient is Polynomial([]), of degree -1 (univariate.py:8-9, 83-84), which matches b_c = -1 only.
-        ok = all(b >= -1 for b in self.bounds)
-        for g, (_, idx, qlen) in enumerate(self.groups):
-            at = [j * qlen + self.bounds[c] for j, c in enumerate(idx) if self.bounds[c] >= 0]
-            if at:
-                vals = eng.gather_batch(quots[g].reshape(1, -1, 2), at).reshape(-1, 2).tolist()
-                ok = ok and all(int(lo) or int(hi) for lo, hi in vals)
-        assert ok, DEGREE_MISMATCH
+            def rows_of(b):
+                rows = [None] * len(self.constraints)
+                for g, (_, idx, _) in enumerate(self.groups):
+                    for j, c in enumerate(idx):
+                        rows[c] = (quots[g][b, j, :max(0, self.bounds[c] + 1)], self.bounds[c])
+                return rows
+            return rows_of, degree_check
 
-        # the combination (:127-146), FRI (:149) and the boundary and randomizer openings (:152-167)
-        rows = [None] * len(self.constraints)
-        for g, (_, idx, _) in enumerate(self.groups):
-            for j, c in enumerate(idx):
-                rows[c] = (quots[g][j, :max(0, self.bounds[c] + 1)], self.bounds[c])
-        self._combine_prove_open(eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_stream)
-        return proof_stream.serialize()
+        streams, _ = self._prove_batch(list(traces), list(boundaries), proof_streams, transition)
+        return [ps.serialize() for ps in streams]
 
 
 def prove_plain(stark, trace, transition_constraints, boundary, proof_stream=None):
     """Stark.prove's signature and result through a PlainStarkPlan built for this one call (no plan is cached)"""
     return PlainStarkPlan(stark, transition_constraints).prove(trace, boundary, proof_stream)
+
+
+def sign_batch(signer, sk, documents):
+    """For an RPSSS or FastRPSSS instance `signer`, [signer.sign(sk, d) for d in documents]: each signature is the
+    one signer.sign gives from the same draws, taken in prove_batch's order (signing draws nothing outside its
+    prove).  The hash, the trace, the boundary and the transition constraints are computed once, one plan proves
+    every document (PlainStarkPlan for a Stark, StarkPlan with the signer's zerofier for a FastStark), and each
+    document's stream is the signer module's own SignatureProofStream.  Nothing is kept between calls."""
+    import sys
+    documents = list(documents)
+    if not documents:
+        return []
+    rp, stark = signer.rp, signer.stark
+    output = rp.hash(sk)
+    trace = rp.trace(sk)
+    transition = rp.transition_constraints(stark.omicron)
+    boundary = rp.boundary_constraints(output)
+    stream = sys.modules[type(signer).__module__].SignatureProofStream
+    streams = [stream(d) for d in documents]
+    if hasattr(signer, "transition_zerofier"):
+        plan = StarkPlan(stark, transition, signer.transition_zerofier)
+        return plan.prove_batch([trace] * len(documents), [boundary] * len(documents),
+                                signer.transition_zerofier_codeword, streams)
+    plan = PlainStarkPlan(stark, transition)
+    return plan.prove_batch([trace] * len(documents), [boundary] * len(documents), streams)
 
 
 _originals = {}  # class -> its own `prove` attribute before enable (None: inherited)
