@@ -176,6 +176,40 @@ int sa_interp_apply_batch(void *out, const void *plan, const void *values, size_
  * k > 2^20.  Host-only: no CUDA call.                                                         */
 size_t sa_interp_batch_max(size_t k);
 
+/* ---- Geometric interpolation plans: interpolation over, and the zerofier of, the domain
+ * 1, step, step^2, ..., step^(k-1), by the closed forms of the q-binomial theorem and two cyclic
+ * convolutions of length K = 2^ceil(log2 2k) (DESIGN section 3.12).  No subproduct tree and no list
+ * of points: k up to 2^26, where the tree stops at 2^20.  The coefficients are those sa_interp_apply
+ * and sa_zerofier give over the explicit domain, bit for bit.
+ * The method needs step^d != 1 for 1 <= d <= k and, from k = 2 on, step != 0.  d < k is "the points
+ * are distinct"; d = k is one more condition: a step of order exactly k (the domain is a whole
+ * subgroup, whose interpolation is an inverse NTT) is refused here although the tree interpolates it.
+ * sa_geo_plan_bytes: the size of a plan, laid out by k alone: 16*(2*sec16(k) + 2K) bytes (96 MiB at
+ * k = 2^20, where the tree's plan is 656 MiB); 0 when k == 0 or k > 2^26.  Host-only: no CUDA call. */
+size_t sa_geo_plan_bytes(size_t k);
+/* Builds the plan of (step, k) into a device buffer of sa_geo_plan_bytes(k) bytes the caller owns.
+ * Before any launch: SA_ESIZE for k outside 1..2^26, SA_EDIVZERO for step == 0 with k >= 2.  After
+ * the build's one synchronisation (it reads the zero flag): SA_EDIVZERO when step^d == 1 for some
+ * 1 <= d <= k, k >= 2 (a single point is never refused); the plan's contents are then unspecified.  */
+int sa_geo_plan(void *plan, const uint64_t step[2], size_t k, void *stream);
+/* out[b*k .. b*k+k) = the coefficients of the polynomial of degree < k that takes values[b*k + i] at
+ * step^i, b < batch, over a plan of (step, k); k must be the plan's.  Rows are contiguous; out must
+ * not overlap values.  SA_ESIZE for k outside 1..2^26 before any launch; batch == 0 returns SA_OK
+ * without a launch.  The promises of sa_interp_apply_batch: the plan is only read (one plan may serve
+ * several streams at once), no host synchronisation, and no allocation once the stream's workspaces
+ * have grown for this k and chunk size, so the call can be captured in a CUDA graph.  The batch runs
+ * in chunks of sa_geo_batch_max(k) vectors, each issuing the launches of one vector: four kernels,
+ * four batched transforms and one strided copy.  A chunk takes 32 bytes per slot (2K per vector) of
+ * per-stream workspace and 16 of the transforms' intermediate.                                    */
+int sa_geo_interp_batch(void *out, const void *plan, const void *values, size_t k, size_t batch, void *stream);
+/* The most vectors one chunk of sa_geo_interp_batch takes: max(1, floor(2^30 / (48 K))) (10 at
+ * k = 2^20), 0 when k == 0 or k > 2^26.  Host-only: no CUDA call.                                 */
+size_t sa_geo_batch_max(size_t k);
+/* out[0..k] = the coefficients of prod_{i<k} (X - step^i) (monic), with sa_geo_plan's limits and
+ * refusals.  Synchronises once, to read the zero flag, before it writes out: an error leaves out
+ * untouched.                                                                                     */
+int sa_geo_zerofier(void *out, const uint64_t step[2], size_t k, void *stream);
+
 /* ---- code/ntt.py:137-176 fast_coset_divide, many numerators over one divisor, and ntt.py:132-135
  * fast_coset_evaluate, many polynomials in one call ------------------------------------------------
  * n = 2^log_n, log_n in [1, 30]; `root` a primitive n-th root of unity (checked like sa_ntt's, before

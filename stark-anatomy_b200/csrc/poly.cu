@@ -2,7 +2,8 @@
 // direct zerofier and Lagrange kernels, the kernels of the subproduct tree (poly_tree.cuh) behind
 // sa_zerofier, sa_interpolate and sa_poly_eval, and those of coset division plans, batched coset
 // evaluation and coset combinations (coset.cuh), of transition quotients (air.cuh) and of boundary quotients
-// (boundary.cuh), with the backend that launches them for the headers' schedules.
+// (boundary.cuh) and of geometric interpolation plans and zerofiers (geo.cuh), with the backend that launches them for
+// the headers' schedules.
 //
 // Reference behaviour reproduced (bit-exact): code/ntt.py:61-176, code/algebra.py:53-57,75-94.
 #include <algorithm>
@@ -10,6 +11,7 @@
 #include "air.cuh"
 #include "boundary.cuh"
 #include "coset.cuh"
+#include "geo.cuh"
 #include "ntt_tile.cuh"
 #include "poly_tree.cuh"
 #include "runtime.cuh"
@@ -249,6 +251,32 @@ __global__ void k_air_store_exact(fe *out, uint32_t *flags, const fe *ws, const 
         if (bad && boundary_flag_leader(ballot, threadIdx.x & 31, log_n)) atomicOr(flags + (idx >> log_n), 1u);
     });
 }
+// ---- geometric plans and zerofiers: each runs its element function of geo.cuh over its index range ----
+__global__ void k_geo_scan_runs(fe *x, long long n, fe *tot) {
+    grid_stride((n + GEO_SCAN_RUN - 1) / GEO_SCAN_RUN, [&](long long r) { geo_scan_run_elem(x, n, tot, r); });
+}
+__global__ void k_geo_scan_add(fe *x, long long n, const fe *tot) {
+    grid_stride(n - GEO_SCAN_RUN, [&](long long idx) { geo_scan_add_elem(x, tot, idx); });
+}
+__global__ void k_geo_factor(fe *P, const fe *pw_m, long long count) {
+    grid_stride(count, [&](long long m) { geo_factor_elem(P, pw_m, m); });
+}
+__global__ void k_geo_seed(fe *out, const fe *pw_m, long long n, long long len) {
+    grid_stride(len, [&](long long t) { geo_seed_elem(out, pw_m, n, t); });
+}
+__global__ void k_geo_zerofier(fe *z, const fe *chirp_m, const fe *P_m, const fe *iP, long long k, int canon,
+                               long long len) {
+    grid_stride(len, [&](long long i) { geo_zerofier_elem(z, chirp_m, P_m, iP, k, canon, i); });
+}
+__global__ void k_geo_weight(fe *c, const fe *iP, long long k) {
+    grid_stride(k, [&](long long i) { geo_weight_elem(c, iP, k, i); });
+}
+__global__ void k_geo_load(fe *ws, const fe *values, const fe *c_m, long long k, int logK, long long batch) {
+    grid_stride(batch << logK, [&](long long idx) { geo_load_elem(ws, values, c_m, k, logK, idx); });
+}
+__global__ void k_geo_mid(fe *dst, const fe *src, const fe *ic_m, long long k, int logK, long long batch) {
+    grid_stride(batch << logK, [&](long long idx) { geo_mid_elem(dst, src, ic_m, k, logK, idx); });
+}
 
 extern "C" {
 
@@ -380,6 +408,25 @@ struct DeviceBoundary : DeviceAir {
 struct DeviceAirExact : DeviceBoundary {
     int air_store_exact(fe *o, uint32_t *flags, const fe *ws, const fe *ipw, ll q, ll tail, int lg, ll nb) {
         return go(k_air_store_exact, tree_grid(nb << lg), o, flags, ws, ipw, q, tail, lg, nb);
+    }
+};
+// DeviceTree plus the launches of the geometric schedules (geo.cuh)
+struct DeviceGeo : DeviceTree {
+    int geo_scan_runs(fe *x, ll n, fe *tot) {
+        return go(k_geo_scan_runs, tree_grid((n + GEO_SCAN_RUN - 1) / GEO_SCAN_RUN), x, n, tot);
+    }
+    int geo_scan_add(fe *x, ll n, const fe *tot) { return go(k_geo_scan_add, tree_grid(n - GEO_SCAN_RUN), x, n, tot); }
+    int geo_factor(fe *P, const fe *pw, ll count) { return go(k_geo_factor, tree_grid(count), P, pw, count); }
+    int geo_seed(fe *o, const fe *pw, ll n, ll len) { return go(k_geo_seed, tree_grid(len), o, pw, n, len); }
+    int geo_zerofier(fe *z, const fe *ch, const fe *P, const fe *iP, ll k, int canon, ll len) {
+        return go(k_geo_zerofier, tree_grid(len), z, ch, P, iP, k, canon, len);
+    }
+    int geo_weight(fe *c, const fe *iP, ll k) { return go(k_geo_weight, tree_grid(k), c, iP, k); }
+    int geo_load(fe *ws, const fe *v, const fe *c, ll k, int lK, ll nb) {
+        return go(k_geo_load, tree_grid(nb << lK), ws, v, c, k, lK, nb);
+    }
+    int geo_mid(fe *d, const fe *s, const fe *ic, ll k, int lK, ll nb) {
+        return go(k_geo_mid, tree_grid(nb << lK), d, s, ic, k, lK, nb);
     }
 };
 static int tree_workspace(Tree &t, cudaStream_t st) {
@@ -707,6 +754,60 @@ int sa_boundary_quotients(void *quot, void *codewords, uint32_t *flags, const vo
     DeviceBoundary b{{{st}}};
     return boundary_quotients(b, (fe *)quot, (fe *)codewords, flags, (const fe *)plan, (const fe *)trace, nregs, ncoef,
                               log_n, root, ws);
+}
+
+// ---- geometric interpolation plans and zerofiers (geo.cuh) ----
+size_t sa_geo_plan_bytes(size_t k) { return sizeof(fe) * geo_plan_layout(k).elems; }
+
+size_t sa_geo_batch_max(size_t k) { return geo_batch_max(k); }
+
+// scratch: the build's workspace (WS_GEO) and the zero flag (WS_PLAN_FLAG)
+int sa_geo_plan(void *plan, const uint64_t step[2], size_t k, void *stream) {
+    SA_TRY(geo_check(k, step));
+    cudaStream_t st = (cudaStream_t)stream;
+    int *flag = nullptr;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&flag, 16, st, WS_PLAN_FLAG));
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * geo_work_layout(k, geo_chirp_len(k, true)).elems, st, WS_GEO));
+    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+    DeviceGeo b{{st}};
+    SA_TRY(geo_plan_build(b, (fe *)plan, step, k, ws, flag));
+    int h = 0;
+    SA_CUDA(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SA_CUDA(cudaStreamSynchronize(st));
+    return h ? SA_EDIVZERO : SA_OK;
+}
+
+// Reads the plan only; its scratch is the stream's workspace (WS_INTERP_APPLY): 2K elements per vector of a chunk
+int sa_geo_interp_batch(void *out, const void *plan, const void *values, size_t k, size_t batch, void *stream) {
+    if (geo_plan_layout(k).elems == 0) return SA_ESIZE;
+    if (batch == 0) return SA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    fe *ws = nullptr;
+    const size_t K = (size_t)geo_plan_layout(k).K, chunk = geo_batch_max(k);
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * 2 * K * std::min(batch, chunk), st, WS_INTERP_APPLY));
+    DeviceGeo b{{st}};
+    return geo_apply(b, (fe *)out, (const fe *)plan, (const fe *)values, k, batch, ws, chunk);
+}
+
+// scratch: the build's workspace and the chirp (WS_GEO) and the zero flag (WS_PLAN_FLAG); the flag is read before the
+// coefficients are written, so an error leaves out untouched
+int sa_geo_zerofier(void *out, const uint64_t step[2], size_t k, void *stream) {
+    SA_TRY(geo_check(k, step));
+    cudaStream_t st = (cudaStream_t)stream;
+    int *flag = nullptr;
+    fe *ws = nullptr;
+    SA_TRY(get_workspace((void **)&flag, 16, st, WS_PLAN_FLAG));
+    SA_TRY(get_workspace((void **)&ws, sizeof(fe) * (geo_work_layout(k, geo_chirp_len(k, false)).elems + k + 1), st,
+                         WS_GEO));
+    SA_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+    DeviceGeo b{{st}};
+    return geo_zerofier(b, (fe *)out, step, k, ws, flag, [&](int *f) -> int {
+        int h = 0;
+        SA_CUDA(cudaMemcpyAsync(&h, f, sizeof(int), cudaMemcpyDeviceToHost, st));
+        SA_CUDA(cudaStreamSynchronize(st));
+        return h ? SA_EDIVZERO : SA_OK;
+    });
 }
 
 }  // extern "C"

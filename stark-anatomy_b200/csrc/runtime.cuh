@@ -88,7 +88,8 @@ enum WsTag {
     WS_INTERP_PLAN = 9,    // sa_interpolate's plan
     WS_INTERP_APPLY = 10,  // an apply's scratch
     WS_COSET = 11,         // coset division and evaluation (coset.cuh): the transformed rows, or offset^i
-    WS_AIR = 12            // transition quotients (air.cuh): the trace's extension and a chunk's quotient rows
+    WS_AIR = 12,           // transition quotients (air.cuh): the trace's extension and a chunk's quotient rows
+    WS_GEO = 13            // a geometric plan's or zerofier's build (geo.cuh): q^t, (q;q)_m, inverses, scan levels
 };
 int get_workspace(void **out, size_t bytes, cudaStream_t st, WsTag tag);
 void keep_pool_memory();

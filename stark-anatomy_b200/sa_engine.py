@@ -59,6 +59,11 @@ SYMBOLS = [
     ("sa_interp_apply", _ci, [_vp, _vp, _vp, _sz, _vp]),
     ("sa_interp_apply_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _vp]),
     ("sa_interp_batch_max", _sz, [_sz]),
+    ("sa_geo_plan_bytes", _sz, [_sz]),
+    ("sa_geo_plan", _ci, [_vp, _u64p, _sz, _vp]),
+    ("sa_geo_interp_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _vp]),
+    ("sa_geo_batch_max", _sz, [_sz]),
+    ("sa_geo_zerofier", _ci, [_vp, _u64p, _sz, _vp]),
     ("sa_coset_div_plan_bytes", _sz, [_ci]),
     ("sa_coset_div_plan", _ci, [_vp, _vp, _sz, _ci, _u64p, _u64p, _vp]),
     ("sa_coset_div_apply_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _ci, _u64p, _sz, _vp]),
@@ -132,6 +137,17 @@ class InterpPlan:
 
     def __init__(self, plan, k):
         self.plan = plan
+        self.k = k
+
+
+class GeoInterpPlan:
+    """A geometric interpolation plan (CudaEngine.geo_interp_plan): the device buffer sa_geo_plan filled (torch.uint8)
+    for the domain step^0 .. step^(k-1)."""
+    __slots__ = ("plan", "step", "k")
+
+    def __init__(self, plan, step, k):
+        self.plan = plan
+        self.step = step
         self.k = k
 
 
@@ -384,6 +400,40 @@ class CudaEngine:
         if batch:
             self._check(self.lib.sa_interp_apply_batch(out.data_ptr(), plan.plan.data_ptr(), values.data_ptr(), plan.k,
                                                        batch, self._stream()))
+        return out
+
+    def tree_fits(self, k):
+        """whether the subproduct tree takes k points (sa_interp_plan_bytes(k) != 0; sa_zerofier has the same cap,
+        2^20): host-only, no CUDA call.  Above it, geometric domains take geo_interp_plan and geo_zerofier."""
+        return self.lib.sa_interp_plan_bytes(k) != 0
+
+    def geo_interp_plan(self, step, k):
+        """sa_geo_plan: what interpolation over step^0 .. step^(k-1) needs of the domain alone, kept on the device for
+        geo_interp_apply (synchronises; "unsupported size" outside 1 <= k <= 2^26, "divide by zero" from k = 2 on
+        when step is 0 or step^d = 1 for some d <= k)"""
+        step = int(step) % P
+        plan = self.torch.empty(max(1, self.lib.sa_geo_plan_bytes(k)), dtype=self.torch.uint8, device=self.device)
+        self._check(self.lib.sa_geo_plan(plan.data_ptr(), _limbs(step), k, self._stream()))
+        return GeoInterpPlan(plan, step, k)
+
+    def geo_interp_apply(self, plan, values):
+        """sa_geo_interp_batch: the coefficients interp_apply gives over the explicit domain, for one vector (k, 2) or
+        a batch of them (B, k, 2) in one call; asynchronous, the plan is only read"""
+        if values.dim() not in (2, 3) or tuple(values.shape[-2:]) != (plan.k, 2):
+            raise SaError(SA_ERRORS[-6])
+        values = values.contiguous()
+        out = self.torch.empty(values.shape, dtype=self.torch.int64, device=self.device)
+        batch = values.shape[0] if values.dim() == 3 else 1
+        if batch:
+            self._check(self.lib.sa_geo_interp_batch(out.data_ptr(), plan.plan.data_ptr(), values.data_ptr(), plan.k,
+                                                     batch, self._stream()))
+        return out
+
+    def geo_zerofier(self, step, k):
+        """sa_geo_zerofier: the k + 1 coefficients of prod_{i<k} (x - step^i), as zerofier gives them over the explicit
+        domain (synchronises once; the refusals of geo_interp_plan)"""
+        out = self.empty(k + 1)
+        self._check(self.lib.sa_geo_zerofier(out.data_ptr(), _limbs(int(step) % P), k, self._stream()))
         return out
 
     @staticmethod

@@ -81,6 +81,13 @@ def _value(lo, hi):
     return (int(lo) & 0xFFFFFFFFFFFFFFFF) | (int(hi) & 0xFFFFFFFFFFFFFFFF) << 64
 
 
+def _tree_fits(eng, k):
+    """whether the engine's subproduct tree takes k points; an engine without the query takes every k up to its
+    MAX_DIRECT_POINTS"""
+    fits = getattr(eng, "tree_fits", None)
+    return fits(k) if fits is not None else k <= eng.MAX_DIRECT_POINTS
+
+
 def _degree(values):
     d = -1
     for i, v in enumerate(values):
@@ -144,10 +151,11 @@ class _Constraint:
 
 class _Stages:
     """The stages FastStark's and Stark's provers share (fast_stark.py:82-106, 116-125, 129-169; stark.py:79-104,
-    113-123, 127-167): the trace randomizers and one batched interpolation, the boundary quotients into the first
-    nregs rows of the commitment buffer, the randomizer polynomial next to them and one commitment of all nregs + 1
-    codewords, the weights, the combination, FRI on the device codeword and the openings of the committed codewords.
-    A plan sets stark, fri, nregs, ncycles, trace_length, log_n, max_degree and interp."""
+    113-123, 127-167): the trace randomizers and one batched interpolation (over the subproduct tree's plan up to its
+    cap, the geometric plan of (omicron, T) above it), the boundary quotients into the first nregs rows of the
+    commitment buffer, the randomizer polynomial next to them and one commitment of all nregs + 1 codewords, the
+    weights, the combination, FRI on the device codeword and the openings of the committed codewords.  A plan sets
+    stark, fri, nregs, ncycles, trace_length, log_n, max_degree and interp."""
 
     def _setup(self, stark, n):
         """fri (the drop-in Fri of the FRI domain of n points) and interp (the randomized trace domain's plan)"""
@@ -156,8 +164,12 @@ class _Stages:
         self.fri = fri if isinstance(fri, _fri.Fri) else _fri.Fri(
             stark.generator, stark.omega, n, stark.expansion_factor, stark.num_colinearity_checks)
         omicron = stark.omicron.value
-        domain = [FieldElement(pow(omicron, i, P), stark.field) for i in range(self.trace_length)]
-        self.interp = eng.interp_plan(eng.upload(sa_devlist.pack(domain)))
+        if _tree_fits(eng, self.trace_length):
+            domain = [FieldElement(pow(omicron, i, P), stark.field) for i in range(self.trace_length)]
+            self.interp = eng.interp_plan(eng.upload(sa_devlist.pack(domain)))
+        else:
+            # above the tree's cap the domain's closed forms: no list of points (DESIGN section 3.12)
+            self.interp = eng.geo_interp_plan(omicron, self.trace_length)
 
     def _trace_polynomials(self, eng, traces):
         """every proof's trace randomizers, drawn proof by proof and row by row in the reference's order (the
@@ -172,8 +184,10 @@ class _Stages:
             rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
                                   for k in range(stark.num_randomizers)]
             values += [rows[c][s] for s in range(nregs) for c in range(T)]
-        columns = eng.upload(sa_devlist.pack(values))
-        return eng.interp_apply(self.interp, columns.reshape(len(traces) * nregs, T, 2))
+        columns = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, T, 2)
+        if isinstance(self.interp, sa_engine.GeoInterpPlan):
+            return eng.geo_interp_apply(self.interp, columns)
+        return eng.interp_apply(self.interp, columns)
 
     def _boundary(self, eng, polys, boundaries, failed):
         """(the (B, nregs + 1, n, 2) commitment buffer with each proof's boundary codewords in its first rows, the
@@ -512,9 +526,9 @@ def prove(stark, trace, transition_constraints, boundary, transition_zerofier, t
 class PlainStarkPlan(_Stages):
     """What does not change between proofs of one AIR on one Stark (stark.py's plain prover): the interpolation plan
     of the randomized trace domain, the transition zerofier built on the device over omicron^0 .. omicron^(ncycles -
-    2) (Stark has no preprocess), one AIR plan per division order, and the constraints' bounds.  Stark keeps neither
-    the omicron domain's nor the FRI domain's length as attributes: they come from len(stark.omicron_domain) and
-    stark.fri.domain_length.  Only read by ``prove``.
+    2) (Stark has no preprocess; by the tree up to its cap, by geo_zerofier above), one AIR plan per division order,
+    and the constraints' bounds.  Stark keeps neither the omicron domain's nor the FRI domain's length as attributes:
+    they come from len(stark.omicron_domain) and stark.fri.domain_length.  Only read by ``prove``.
 
     The reference divides each transition numerator by Polynomial.__truediv__, an exact division, so the division
     order never changes its result: constraint c (numerator degree bound D_c, T the randomized trace length) divides
@@ -558,8 +572,11 @@ class PlainStarkPlan(_Stages):
         self.groups = []  # (AirPlan, constraint indices, qlen)
         if self.ncycles < 2:
             return
-        points = [FieldElement(pow(omicron, i, P), field) for i in range(self.ncycles - 1)]
-        self.zerofier = eng.zerofier(eng.upload(sa_devlist.pack(points)))
+        if _tree_fits(eng, self.ncycles - 1):
+            points = [FieldElement(pow(omicron, i, P), field) for i in range(self.ncycles - 1)]
+            self.zerofier = eng.zerofier(eng.upload(sa_devlist.pack(points)))
+        else:
+            self.zerofier = eng.geo_zerofier(omicron, self.ncycles - 1)
         for order in sorted(set(orders)):
             idx = [c for c, o in enumerate(orders) if o == order]
             plan = eng.air_plan([self.constraints[c] for c in idx], nregs, self.zerofier, T, order.bit_length() - 1,
