@@ -468,6 +468,20 @@ int sa_fri_commit(void *layers, void *trees, const void *codeword, size_t n, int
                   const uint64_t offset[2], const uint64_t omega[2], sa_fri_challenge_fn challenge, void *user,
                   void *stream);
 
+/* ---- seeded randomizer draws (code/algebra.py:118-120 field.sample(os.urandom(17))) -------------
+ * For a 32-byte seed s, draw j (a uint64) is the element field.sample gives when os.urandom(17) returns
+ * blake2b(s || j as 8 little-endian bytes).digest()[:17] (64-byte digest, no key): that digest's first 17 bytes
+ * read big-endian, mod p (DESIGN section 3.13).  For seed b (the 32 bytes at seeds + 32*b, device memory, no
+ * alignment needed) and j < count, the element of draw first + j is written at element offset
+ *     b*seed_stride + (j % width)*lane_stride + j / width
+ * of out; no other element is touched.  With width = nregs and lane_stride = T this fills the randomizer rows of
+ * register-major trace columns; with width = 1 it writes count consecutive elements per seed.  nseeds == 0 or
+ * count == 0 returns SA_OK without a launch.  Before any launch: SA_ESIZE for width == 0, for first + count - 1
+ * above 2^64 - 1, and for an item count nseeds*count or a largest offset at or above 2^59 elements.  One launch,
+ * no allocation; asynchronous and graph-capturable.                                                       */
+int sa_sample_seeded(void *out, const void *seeds, size_t nseeds, size_t seed_stride, uint64_t first, size_t count,
+                     size_t width, size_t lane_stride, void *stream);
+
 /* ---- device memory the library keeps between calls (no reference counterpart) ------------------
  * Twiddle tables (per device, log n, root, direction) and FRI x^-1 tables (per device, omega, n)
  * live in one least-recently-used cache bounded by bytes: default 4 GiB, SA_CACHE_LIMIT_MIB, or

@@ -96,6 +96,7 @@ SYMBOLS = [
     ("sa_gather_batch", _ci, [_vp, _vp, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_merkle_open_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_gather_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
+    ("sa_sample_seeded", _ci, [_vp, _vp, _sz, _sz, ctypes.c_uint64, _sz, _sz, _sz, _vp]),
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_commit", _ci, [_vp, _vp, _vp, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
@@ -841,6 +842,44 @@ class CudaEngine:
             self._count("h2d", 8 * len(flat))
             self._count("d2h", out.numel() * 8)
         return out.cpu().numpy()
+
+    # --------------------------------------------------------------- sample
+    def upload_seeds(self, seeds):
+        """a list of 32-byte `bytes` -> one (nseeds, 32) uint8 device tensor (one upload); "unsupported size" for
+        anything else"""
+        if not all(isinstance(s, bytes) and len(s) == 32 for s in seeds):
+            raise SaError(SA_ERRORS[-6])
+        torch = self.torch
+        if not seeds:
+            return torch.empty((0, 32), dtype=torch.uint8, device=self.device)
+        host = torch.frombuffer(bytearray(b"".join(seeds)), dtype=torch.uint8).reshape(-1, 32)
+        self._count("h2d", host.numel())
+        return host.to(self.device)
+
+    def sample_seeded(self, out, seeds, first, count, width=1, lane_stride=1, seed_stride=None, offset=0):
+        """sa_sample_seeded into the contiguous int64 tensor `out` (..., 2) from element `offset` on: for seed b and
+        j < count, the element of draw first + j (DESIGN section 3.13) at offset + b seed_stride + (j % width)
+        lane_stride + j // width.  `seeds` is a list of 32-byte bytes (upload_seeds) or the (nseeds, 32) uint8 device
+        tensor it gives; seed_stride defaults to count.  Asynchronous; "unsupported size" before any device work for
+        width 0 or when the largest offset falls outside `out`.  Returns out."""
+        torch = self.torch
+        if not isinstance(seeds, torch.Tensor):
+            seeds = self.upload_seeds(list(seeds))
+        if (seeds.dtype != torch.uint8 or seeds.dim() != 2 or seeds.shape[1] != 32 or not seeds.is_contiguous()
+                or out.dtype != torch.int64 or out.shape[-1] != 2 or not out.is_contiguous()):
+            raise SaError(SA_ERRORS[-6])
+        nseeds = seeds.shape[0]
+        seed_stride = count if seed_stride is None else seed_stride
+        if width < 1 or min(first, count, lane_stride, seed_stride, offset) < 0 or first + count > 1 << 64:
+            raise SaError(SA_ERRORS[-6])
+        if nseeds == 0 or count == 0:
+            return out
+        last = offset + (nseeds - 1) * seed_stride + (min(count, width) - 1) * lane_stride + (count - 1) // width
+        if last >= out.numel() // 2:
+            raise SaError(SA_ERRORS[-6])
+        self._check(self.lib.sa_sample_seeded(out.data_ptr() + 16 * offset, seeds.data_ptr(), nseeds, seed_stride,
+                                              first, count, width, lane_stride, self._stream()))
+        return out
 
     # ------------------------------------------------------------------ fri
     def fri_fold(self, vec, alpha, offset, omega):

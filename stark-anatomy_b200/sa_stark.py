@@ -33,10 +33,15 @@ combination into one codeword per proof, one gather and one path read for all op
 proof is the bytes ``prove`` gives from the same draws (DESIGN section 3.11); ``prove`` is ``prove_batch`` of one.
 ``sign_batch`` signs many documents with one key on an RPSSS or FastRPSSS instance.
 
+With a 32-byte ``seed`` per proof (``prove(..., seed=)``, ``prove_batch(..., seeds=)``, ``sign_batch(..., seeds=)``)
+the randomizers are expanded from the seed on the device (``sample_seeded``, DESIGN section 3.13) and nothing calls
+os.urandom: the proof is the one the unseeded prover gives with os.urandom = ``seeded_urandom(seed)``.
+
 ``enable(cls)`` rebinds ``cls.prove`` (FastStark's) to ``prove``, ``enable_plain(cls)`` rebinds Stark's to
 ``prove_plain``; ``disable()`` restores both.  Off by default, as ``sa_accel``.  Nothing here imports torch or holds
 device state outside a plan.
 """
+import itertools
 import os
 from hashlib import blake2b
 
@@ -94,6 +99,27 @@ def _degree(values):
         if v:
             d = i
     return d
+
+
+def _seeds(seeds, count):
+    """None, or the list of one 32-byte ``bytes`` seed (a list or tuple) for each of `count` proofs"""
+    assert seeds is None or (isinstance(seeds, (list, tuple)) and len(seeds) == count and
+                             all(isinstance(s, bytes) and len(s) == 32 for s in seeds)), \
+        "sa_stark: seeds must be a list of one 32-byte bytes object per proof"
+    return None if seeds is None else list(seeds)
+
+
+def seeded_urandom(seed):
+    """os.urandom for one seeded proof: the n-th call returns blake2b(seed || n as 8 little-endian bytes)'s first 17
+    bytes, the draw the device expands for draw n (DESIGN section 3.13).  With os.urandom replaced by it, the unseeded
+    prover (or the reference's own prove) gives the seeded proof's bytes.  Only os.urandom(17) is served."""
+    assert isinstance(seed, bytes) and len(seed) == 32, "sa_stark: a seed is 32 bytes"
+    counter = itertools.count()
+
+    def urandom(n):
+        assert n == 17, "sa_stark: seeded_urandom serves the provers' 17-byte draws only, not %r bytes" % (n,)
+        return blake2b(seed + next(counter).to_bytes(8, "little")).digest()[:17]
+    return urandom
 
 
 class Params:
@@ -171,20 +197,30 @@ class _Stages:
             # above the tree's cap the domain's closed forms: no list of points (DESIGN section 3.12)
             self.interp = eng.geo_interp_plan(omicron, self.trace_length)
 
-    def _trace_polynomials(self, eng, traces):
+    def _trace_polynomials(self, eng, traces, seeds=None):
         """every proof's trace randomizers, drawn proof by proof and row by row in the reference's order (the
         callers' lists are not touched), one upload of all columns and one batched interpolation: the (B nregs, T, 2)
-        trace polynomials, proof b's register s in row b nregs + s"""
+        trace polynomials, proof b's register s in row b nregs + s.  With `seeds` (the (B, 32) device seeds) only the
+        callers' rows are uploaded, and one sample_seeded launch writes row k of register s of proof b as draw
+        k nregs + s of seed b (DESIGN section 3.13)"""
         stark, field, nregs, T = self.stark, self.stark.field, self.nregs, self.trace_length
         for trace in traces:
             assert len(trace) == self.ncycles, \
                 "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
-        values = []
-        for trace in traces:
-            rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
-                                  for k in range(stark.num_randomizers)]
-            values += [rows[c][s] for s in range(nregs) for c in range(T)]
-        columns = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, T, 2)
+        if seeds is None:
+            values = []
+            for trace in traces:
+                rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
+                                      for k in range(stark.num_randomizers)]
+                values += [rows[c][s] for s in range(nregs) for c in range(T)]
+            columns = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, T, 2)
+        else:
+            ncycles = self.ncycles
+            values = [trace[c][s] for trace in traces for s in range(nregs) for c in range(ncycles)]
+            columns = eng.empty(len(traces) * nregs * T).reshape(len(traces) * nregs, T, 2)
+            columns[:, :ncycles] = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, ncycles, 2)
+            eng.sample_seeded(columns, seeds, 0, stark.num_randomizers * nregs, width=nregs, lane_stride=T,
+                              seed_stride=nregs * T, offset=ncycles)
         if isinstance(self.interp, sa_engine.GeoInterpPlan):
             return eng.geo_interp_apply(self.interp, columns)
         return eng.interp_apply(self.interp, columns)
@@ -233,24 +269,29 @@ class _Stages:
         field = self.stark.field
         return [[field.sample(os.urandom(17)) for i in range(self.max_degree + 1)] for b in range(count)]
 
-    def _commit(self, eng, committed, randomizers, proof_streams):
-        """every proof's randomizer codeword in its last row of the buffer (one batched coset_evaluate), one
-        commitment of all B (nregs + 1) rows, and each proof's roots pushed in order into its stream: (the (B,
-        max_degree + 1, 2) randomizers, the trees)"""
-        stark, nregs, log_n, B = self.stark, self.nregs, self.log_n, len(randomizers)
-        rvec = eng.upload(sa_devlist.pack([r for rs in randomizers for r in rs]))
+    def _seeded_randomizers(self, eng, seeds):
+        """the (B, max_degree + 1, 2) randomizer polynomials from one sample_seeded launch: coefficient i of proof b
+        is draw num_randomizers nregs + i of seed b, the draw after its trace randomizers"""
+        width = self.max_degree + 1
+        rvec = eng.empty(seeds.shape[0] * width).reshape(seeds.shape[0], width, 2)
+        eng.sample_seeded(rvec, seeds, self.stark.num_randomizers * self.nregs, width)
+        return rvec
+
+    def _commit(self, eng, committed, rvec, proof_streams):
+        """every proof's randomizer codeword from the (B, max_degree + 1, 2) randomizers `rvec` in its last row of the
+        buffer (one batched coset_evaluate), one commitment of all B (nregs + 1) rows, and each proof's roots pushed in
+        order into its stream: the trees"""
+        stark, nregs, log_n, B = self.stark, self.nregs, self.log_n, rvec.shape[0]
         if B == 1:
-            eng.coset_evaluate(rvec, log_n, stark.omega.value, stark.generator.value, out=committed[0, nregs])
-            rvec = rvec.reshape(1, self.max_degree + 1, 2)
+            eng.coset_evaluate(rvec[0], log_n, stark.omega.value, stark.generator.value, out=committed[0, nregs])
         else:
-            rvec = rvec.reshape(B, self.max_degree + 1, 2)
             committed[:, nregs] = eng.coset_evaluate(rvec, log_n, stark.omega.value, stark.generator.value)
         trees = eng.merkle_trees(committed.reshape(B * (nregs + 1), 1 << log_n, 2))
         roots = eng.tree_roots(trees)
         for b, ps in enumerate(proof_streams):
             for root in roots[b * (nregs + 1):(b + 1) * (nregs + 1)]:
                 ps.push(root)
-        return rvec, trees
+        return trees
 
     def _weights(self, proof_stream):
         """1 + 2 ncons + 2 nregs weights from the caller's prover_fiat_shamir()"""
@@ -308,13 +349,15 @@ class _Stages:
                     ps.push(paths[r][q])
         return quadrupled
 
-    def _prove_batch(self, traces, boundaries, proof_streams, transition):
+    def _prove_batch(self, traces, boundaries, proof_streams, transition, seeds=None):
         """the schedule both provers share: (the proof streams, each proof's quadrupled indices).  transition(eng,
         polys, failed, B) runs the plan's transition quotients and their checks for every proof not yet in `failed`
         and returns (rows_of, degree_check): rows_of(b) gives proof b's combination rows, degree_check(eng, live,
-        failed) checks the proofs below `live`."""
-        eng = sa_engine.get_engine()
+        failed) checks the proofs below `live`.  With `seeds` (one 32-byte seed per proof) every draw comes from the
+        device expansion of its proof's seed and nothing calls os.urandom."""
         B = len(traces)
+        seeds = _seeds(seeds, B)
+        eng = sa_engine.get_engine()
         assert len(boundaries) == B, "sa_stark: %d traces and %d boundaries" % (B, len(boundaries))
         if proof_streams is None:
             proof_streams = [sa_host.ip.ProofStream() for b in range(B)]
@@ -322,13 +365,15 @@ class _Stages:
         if B == 0:
             return [], []
 
-        polys = self._trace_polynomials(eng, traces)
+        seeds_dev = None if seeds is None else eng.upload_seeds(seeds)
+        polys = self._trace_polynomials(eng, traces, seeds_dev)
         failed = {}  # proof -> the exception proving it alone raises first
         stage = self._boundary(eng, polys, boundaries, failed)
         if stage is None:
             # a boundary the plan refuses: the proofs before the lowest such proof run as a batch of their own
             b, exc = self._refused(eng, boundaries)
-            self._prove_batch(traces[:b], boundaries[:b], proof_streams[:b], transition)
+            self._prove_batch(traces[:b], boundaries[:b], proof_streams[:b], transition,
+                              None if seeds is None else seeds[:b])
             exc.proof_index = b
             raise exc
         committed, bquot, bounds_b = stage
@@ -336,9 +381,15 @@ class _Stages:
 
         # the proofs before the lowest failed one go on: their randomizers, and their degree checks
         live = min(failed) if failed else B
-        randomizers = self._randomizers(live)
+        if seeds is None:
+            randomizers = self._randomizers(live)
         if not failed:
-            rvec, trees = self._commit(eng, committed, randomizers, proof_streams)
+            if seeds is None:
+                rvec = eng.upload(sa_devlist.pack([r for rs in randomizers for r in rs]))
+                rvec = rvec.reshape(B, self.max_degree + 1, 2)
+            else:
+                rvec = self._seeded_randomizers(eng, seeds_dev)
+            trees = self._commit(eng, committed, rvec, proof_streams)
             weights = [self._weights(ps) for ps in proof_streams]
         degree_check(eng, live, failed)
         if failed:
@@ -438,18 +489,21 @@ class StarkPlan(_Stages):
             acc += t
         return acc % P
 
-    def prove(self, trace, boundary, transition_zerofier_codeword, proof_stream=None):
+    def prove(self, trace, boundary, transition_zerofier_codeword, proof_stream=None, seed=None):
         """FastStark.prove(trace, constraints, boundary, zerofier, zerofier_codeword, proof_stream) for this plan's
-        constraints and zerofier: proof_stream.serialize().  It is prove_batch of one."""
+        constraints and zerofier: proof_stream.serialize().  It is prove_batch of one; `seed` (32 bytes) draws the
+        randomizers from its device expansion instead of os.urandom."""
         return self.prove_batch([trace], [boundary], transition_zerofier_codeword,
-                                None if proof_stream is None else [proof_stream])[0]
+                                None if proof_stream is None else [proof_stream], None if seed is None else [seed])[0]
 
-    def prove_batch(self, traces, boundaries, transition_zerofier_codeword, proof_streams=None):
+    def prove_batch(self, traces, boundaries, transition_zerofier_codeword, proof_streams=None, seeds=None):
         """FastStark.prove for each (traces[b], boundaries[b], proof_streams[b]) with this plan's constraints and
         zerofier, the pre-FRI stages of all proofs in one schedule: the list of proof bytes, proof b's the bytes
         proving it alone gives from the same draws (DESIGN section 3.11 gives the draw order).  The exception is the
         one proving the proofs one at a time in order raises first, with the failing proof's index as
-        ``proof_index``."""
+        ``proof_index``.  With `seeds`, one 32-byte seed per proof, proof b's draws are the device expansion of
+        seeds[b] (DESIGN section 3.13): its bytes are those proving it alone with os.urandom = seeded_urandom(seeds[b])
+        gives, whatever the batch."""
         T, nregs = self.trace_length, self.nregs
         where = self._where()
 
@@ -498,7 +552,7 @@ class StarkPlan(_Stages):
                 return [(quots[where[k.index][0]][b, where[k.index][1], :k.bound + 1], k.bound) for k in self.cons]
             return rows_of, degree_check
 
-        streams, quadrupled = self._prove_batch(list(traces), list(boundaries), proof_streams, transition)
+        streams, quadrupled = self._prove_batch(list(traces), list(boundaries), proof_streams, transition, seeds)
 
         # ... and the zerofier's openings (:171-175), proof by proof: the codeword is the caller's
         zc = transition_zerofier_codeword
@@ -583,16 +637,18 @@ class PlainStarkPlan(_Stages):
                                 field.primitive_nth_root(order).value, stark.generator.value, omicron)
             self.groups.append((plan, idx, max(1, max(self.bounds[c] for c in idx) + 1)))
 
-    def prove(self, trace, boundary, proof_stream=None):
+    def prove(self, trace, boundary, proof_stream=None, seed=None):
         """Stark.prove(trace, constraints, boundary, proof_stream) for this plan's constraints:
-        proof_stream.serialize().  It is prove_batch of one."""
-        return self.prove_batch([trace], [boundary], None if proof_stream is None else [proof_stream])[0]
+        proof_stream.serialize().  It is prove_batch of one; `seed` as StarkPlan.prove's."""
+        return self.prove_batch([trace], [boundary], None if proof_stream is None else [proof_stream],
+                                None if seed is None else [seed])[0]
 
-    def prove_batch(self, traces, boundaries, proof_streams=None):
+    def prove_batch(self, traces, boundaries, proof_streams=None, seeds=None):
         """Stark.prove for each (traces[b], boundaries[b], proof_streams[b]) with this plan's constraints, the
         pre-FRI stages of all proofs in one schedule: the list of proof bytes, proof b's the bytes proving it alone
         gives from the same draws (DESIGN section 3.11).  The exception is the one proving the proofs one at a time
-        in order raises first, with the failing proof's index as ``proof_index``."""
+        in order raises first, with the failing proof's index as ``proof_index``.  `seeds` as
+        StarkPlan.prove_batch's."""
         T, nregs = self.trace_length, self.nregs
 
         def transition(eng, polys, failed, B):
@@ -640,7 +696,7 @@ class PlainStarkPlan(_Stages):
                 return rows
             return rows_of, degree_check
 
-        streams, _ = self._prove_batch(list(traces), list(boundaries), proof_streams, transition)
+        streams, _ = self._prove_batch(list(traces), list(boundaries), proof_streams, transition, seeds)
         return [ps.serialize() for ps in streams]
 
 
@@ -649,14 +705,17 @@ def prove_plain(stark, trace, transition_constraints, boundary, proof_stream=Non
     return PlainStarkPlan(stark, transition_constraints).prove(trace, boundary, proof_stream)
 
 
-def sign_batch(signer, sk, documents):
+def sign_batch(signer, sk, documents, seeds=None):
     """For an RPSSS or FastRPSSS instance `signer`, [signer.sign(sk, d) for d in documents]: each signature is the
     one signer.sign gives from the same draws, taken in prove_batch's order (signing draws nothing outside its
     prove).  The hash, the trace, the boundary and the transition constraints are computed once, one plan proves
     every document (PlainStarkPlan for a Stark, StarkPlan with the signer's zerofier for a FastStark), and each
-    document's stream is the signer module's own SignatureProofStream.  Nothing is kept between calls."""
+    document's stream is the signer module's own SignatureProofStream.  Nothing is kept between calls.  With
+    `seeds`, one secret 32-byte seed per document, signature d is signer.sign(sk, documents[d]) with os.urandom =
+    seeded_urandom(seeds[d]); a seed must never sign two different documents (DESIGN section 3.13)."""
     import sys
     documents = list(documents)
+    seeds = _seeds(seeds, len(documents))
     if not documents:
         return []
     rp, stark = signer.rp, signer.stark
@@ -669,9 +728,9 @@ def sign_batch(signer, sk, documents):
     if hasattr(signer, "transition_zerofier"):
         plan = StarkPlan(stark, transition, signer.transition_zerofier)
         return plan.prove_batch([trace] * len(documents), [boundary] * len(documents),
-                                signer.transition_zerofier_codeword, streams)
+                                signer.transition_zerofier_codeword, streams, seeds)
     plan = PlainStarkPlan(stark, transition)
-    return plan.prove_batch([trace] * len(documents), [boundary] * len(documents), streams)
+    return plan.prove_batch([trace] * len(documents), [boundary] * len(documents), streams, seeds)
 
 
 _originals = {}  # class -> its own `prove` attribute before enable (None: inherited)
