@@ -482,6 +482,24 @@ int sa_fri_commit(void *layers, void *trees, const void *codeword, size_t n, int
 int sa_sample_seeded(void *out, const void *seeds, size_t nseeds, size_t seed_stride, uint64_t first, size_t count,
                      size_t width, size_t lane_stride, void *stream);
 
+/* ---- Rescue-Prime over many inputs (code/rescue_prime.py:100-203 hash and trace, state width 2) -------------
+ * For b < count, input x = inputs[b] (canonical, device memory): absorb [x, 0], then `rounds` rounds, round r a
+ * forward half-round (S-box s^alpha, MDS, constants 4r + i) and a backward half-round (S-box s^alphainv, MDS,
+ * constants 4r + 2 + i), i < 2.  `constants` (device memory, canonical) is the MDS matrix row-major (4 elements),
+ * then the 4*rounds round constants in the reference's order; the exponents are 128-bit host values, lo word first.
+ * The library holds no Rescue constant of its own.  hashes[b] receives state[0] after the last round (hashes may be
+ * NULL); trace (may be NULL) receives register s of row r <= rounds at element offset
+ *     b*inst_stride + s*lane_stride + r
+ * where row 0 is the absorbed state and row r + 1 the state after round r; no other element is touched.  With
+ * lane_stride = T and inst_stride = 2T this fills rows 0..rounds of register-major trace columns of length T.
+ * count == 0 returns SA_OK without a launch.  Before any launch: SA_ESIZE for both outputs NULL, rounds of 0 or
+ * above SA_RESCUE_MAX_ROUNDS (the constants live in shared memory), and a count or largest element offset at or
+ * above 2^59.  One launch, no allocation; asynchronous and graph-capturable (DESIGN section 3.14).              */
+#define SA_RESCUE_MAX_ROUNDS 512
+int sa_rescue(void *hashes, void *trace, const void *inputs, size_t count, const void *constants, size_t rounds,
+              const uint64_t alpha[2], const uint64_t alphainv[2], size_t inst_stride, size_t lane_stride,
+              void *stream);
+
 /* ---- device memory the library keeps between calls (no reference counterpart) ------------------
  * Twiddle tables (per device, log n, root, direction) and FRI x^-1 tables (per device, omega, n)
  * live in one least-recently-used cache bounded by bytes: default 4 GiB, SA_CACHE_LIMIT_MIB, or

@@ -97,6 +97,7 @@ SYMBOLS = [
     ("sa_merkle_open_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_gather_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_sample_seeded", _ci, [_vp, _vp, _sz, _sz, ctypes.c_uint64, _sz, _sz, _sz, _vp]),
+    ("sa_rescue", _ci, [_vp, _vp, _vp, _sz, _vp, _sz, _u64p, _u64p, _sz, _sz, _vp]),
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_commit", _ci, [_vp, _vp, _vp, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
@@ -880,6 +881,40 @@ class CudaEngine:
         self._check(self.lib.sa_sample_seeded(out.data_ptr() + 16 * offset, seeds.data_ptr(), nseeds, seed_stride,
                                               first, count, width, lane_stride, self._stream()))
         return out
+
+    # --------------------------------------------------------------- rescue
+    RESCUE_MAX_ROUNDS = 512  # SA_RESCUE_MAX_ROUNDS
+
+    def rescue(self, inputs, constants, rounds, alpha, alphainv, hashes=None, trace=None, inst_stride=None,
+               lane_stride=None):
+        """sa_rescue (DESIGN section 3.14): the Rescue-Prime permutation of width 2 over the (count, 2) canonical
+        `inputs` with `rounds` rounds, the exponents alpha and alphainv (ints below 2^128) and the device `constants`
+        (the MDS matrix row-major, then 4 rounds round constants).  hashes[b] gets input b's hash; the contiguous
+        int64 tensor `trace` (..., 2) gets register s of row r <= rounds at b inst_stride + s lane_stride + r
+        (default: dense, lane_stride = rounds + 1 and inst_stride = 2 lane_stride).  Either output may be None, not
+        both.  Asynchronous; "unsupported size" before any device work for both outputs None, rounds outside
+        1..RESCUE_MAX_ROUNDS, an exponent outside 0..2^128 - 1, or a buffer shorter than the call reads or writes.
+        Returns (hashes, trace)."""
+        lane_stride = rounds + 1 if lane_stride is None else lane_stride
+        inst_stride = 2 * lane_stride if inst_stride is None else inst_stride
+        vecs = [v for v in (inputs, constants, hashes, trace) if v is not None]
+        if (any(v.dtype != self.torch.int64 or v.shape[-1] != 2 or not v.is_contiguous() for v in vecs)
+                or (hashes is None and trace is None) or not 1 <= rounds <= self.RESCUE_MAX_ROUNDS
+                or not all(0 <= int(e) < 1 << 128 for e in (alpha, alphainv)) or min(inst_stride, lane_stride) < 0
+                or constants.numel() // 2 < 4 + 4 * rounds):
+            raise SaError(SA_ERRORS[-6])
+        count = inputs.numel() // 2
+        if hashes is not None and hashes.numel() // 2 < count:
+            raise SaError(SA_ERRORS[-6])
+        if trace is not None and count and (count - 1) * inst_stride + lane_stride + rounds >= trace.numel() // 2:
+            raise SaError(SA_ERRORS[-6])
+        if count == 0:
+            return hashes, trace
+        self._check(self.lib.sa_rescue(None if hashes is None else hashes.data_ptr(),
+                                       None if trace is None else trace.data_ptr(), inputs.data_ptr(), count,
+                                       constants.data_ptr(), rounds, _limbs(alpha), _limbs(alphainv), inst_stride,
+                                       lane_stride, self._stream()))
+        return hashes, trace
 
     # ------------------------------------------------------------------ fri
     def fri_fold(self, vec, alpha, offset, omega):

@@ -31,7 +31,9 @@ openings.
 batch (one interpolation, one boundary apply, one transition apply per division order, one commitment, one
 combination into one codeword per proof, one gather and one path read for all openings), FRI runs per proof, and each
 proof is the bytes ``prove`` gives from the same draws (DESIGN section 3.11); ``prove`` is ``prove_batch`` of one.
-``sign_batch`` signs many documents with one key on an RPSSS or FastRPSSS instance.
+``sign_batch`` signs many documents with one key on an RPSSS or FastRPSSS instance; ``SignerPlan`` keeps a signer's
+AIR, plan and Rescue constants and signs under many keys per call, each key's trace computed on the device straight
+into the prover's column buffer (DESIGN section 3.14).
 
 With a 32-byte ``seed`` per proof (``prove(..., seed=)``, ``prove_batch(..., seeds=)``, ``sign_batch(..., seeds=)``)
 the randomizers are expanded from the seed on the device (``sample_seeded``, DESIGN section 3.13) and nothing calls
@@ -49,6 +51,7 @@ import sa_host
 import sa_engine
 import sa_devlist
 import sa_marshal
+import sa_rescue
 import fri as _fri
 
 P = sa_engine.P
@@ -197,30 +200,39 @@ class _Stages:
             # above the tree's cap the domain's closed forms: no list of points (DESIGN section 3.12)
             self.interp = eng.geo_interp_plan(omicron, self.trace_length)
 
-    def _trace_polynomials(self, eng, traces, seeds=None):
+    def _trace_polynomials(self, eng, traces, seeds=None, columns=None):
         """every proof's trace randomizers, drawn proof by proof and row by row in the reference's order (the
         callers' lists are not touched), one upload of all columns and one batched interpolation: the (B nregs, T, 2)
         trace polynomials, proof b's register s in row b nregs + s.  With `seeds` (the (B, 32) device seeds) only the
         callers' rows are uploaded, and one sample_seeded launch writes row k of register s of proof b as draw
-        k nregs + s of seed b (DESIGN section 3.13)"""
+        k nregs + s of seed b (DESIGN section 3.13).  With `columns`, the (B nregs, T, 2) column buffer whose first
+        ncycles rows are already filled on the device, no trace element is uploaded: only its randomizer rows are
+        written, from the same draws"""
         stark, field, nregs, T = self.stark, self.stark.field, self.nregs, self.trace_length
-        for trace in traces:
-            assert len(trace) == self.ncycles, \
-                "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
-        if seeds is None:
-            values = []
+        ncycles, nrand = self.ncycles, stark.num_randomizers
+        if columns is None:
             for trace in traces:
-                rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
-                                      for k in range(stark.num_randomizers)]
-                values += [rows[c][s] for s in range(nregs) for c in range(T)]
-            columns = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, T, 2)
-        else:
-            ncycles = self.ncycles
-            values = [trace[c][s] for trace in traces for s in range(nregs) for c in range(ncycles)]
-            columns = eng.empty(len(traces) * nregs * T).reshape(len(traces) * nregs, T, 2)
-            columns[:, :ncycles] = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, ncycles, 2)
-            eng.sample_seeded(columns, seeds, 0, stark.num_randomizers * nregs, width=nregs, lane_stride=T,
-                              seed_stride=nregs * T, offset=ncycles)
+                assert len(trace) == self.ncycles, \
+                    "sa_stark: a trace of %d rows, the plan is for %d cycles" % (len(trace), self.ncycles)
+            if seeds is None:
+                values = []
+                for trace in traces:
+                    rows = list(trace) + [[field.sample(os.urandom(17)) for s in range(nregs)]
+                                          for k in range(nrand)]
+                    values += [rows[c][s] for s in range(nregs) for c in range(T)]
+                columns = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, T, 2)
+            else:
+                values = [trace[c][s] for trace in traces for s in range(nregs) for c in range(ncycles)]
+                columns = eng.empty(len(traces) * nregs * T).reshape(len(traces) * nregs, T, 2)
+                columns[:, :ncycles] = eng.upload(sa_devlist.pack(values)).reshape(len(traces) * nregs, ncycles, 2)
+        elif seeds is None:
+            B = columns.shape[0] // nregs
+            draws = [[field.sample(os.urandom(17)) for s in range(nregs)] for b in range(B) for k in range(nrand)]
+            values = [draws[b * nrand + k][s] for b in range(B) for s in range(nregs) for k in range(nrand)]
+            columns[:, ncycles:] = eng.upload(sa_devlist.pack(values)).reshape(B * nregs, nrand, 2)
+        if seeds is not None:
+            eng.sample_seeded(columns, seeds, 0, nrand * nregs, width=nregs, lane_stride=T, seed_stride=nregs * T,
+                              offset=ncycles)
         if isinstance(self.interp, sa_engine.GeoInterpPlan):
             return eng.geo_interp_apply(self.interp, columns)
         return eng.interp_apply(self.interp, columns)
@@ -349,13 +361,14 @@ class _Stages:
                     ps.push(paths[r][q])
         return quadrupled
 
-    def _prove_batch(self, traces, boundaries, proof_streams, transition, seeds=None):
+    def _prove_batch(self, traces, boundaries, proof_streams, transition, seeds=None, columns=None):
         """the schedule both provers share: (the proof streams, each proof's quadrupled indices).  transition(eng,
         polys, failed, B) runs the plan's transition quotients and their checks for every proof not yet in `failed`
         and returns (rows_of, degree_check): rows_of(b) gives proof b's combination rows, degree_check(eng, live,
         failed) checks the proofs below `live`.  With `seeds` (one 32-byte seed per proof) every draw comes from the
-        device expansion of its proof's seed and nothing calls os.urandom."""
-        B = len(traces)
+        device expansion of its proof's seed and nothing calls os.urandom.  With `columns` (the (B nregs, T, 2)
+        device column buffer with every proof's trace in its first ncycles rows) `traces` is None."""
+        B = len(traces) if columns is None else len(boundaries)
         seeds = _seeds(seeds, B)
         eng = sa_engine.get_engine()
         assert len(boundaries) == B, "sa_stark: %d traces and %d boundaries" % (B, len(boundaries))
@@ -366,14 +379,15 @@ class _Stages:
             return [], []
 
         seeds_dev = None if seeds is None else eng.upload_seeds(seeds)
-        polys = self._trace_polynomials(eng, traces, seeds_dev)
+        polys = self._trace_polynomials(eng, traces, seeds_dev, columns)
         failed = {}  # proof -> the exception proving it alone raises first
         stage = self._boundary(eng, polys, boundaries, failed)
         if stage is None:
             # a boundary the plan refuses: the proofs before the lowest such proof run as a batch of their own
             b, exc = self._refused(eng, boundaries)
-            self._prove_batch(traces[:b], boundaries[:b], proof_streams[:b], transition,
-                              None if seeds is None else seeds[:b])
+            self._prove_batch(None if columns is not None else traces[:b], boundaries[:b], proof_streams[:b],
+                              transition, None if seeds is None else seeds[:b],
+                              None if columns is None else columns[:b * self.nregs])
             exc.proof_index = b
             raise exc
         committed, bquot, bounds_b = stage
@@ -504,6 +518,10 @@ class StarkPlan(_Stages):
         ``proof_index``.  With `seeds`, one 32-byte seed per proof, proof b's draws are the device expansion of
         seeds[b] (DESIGN section 3.13): its bytes are those proving it alone with os.urandom = seeded_urandom(seeds[b])
         gives, whatever the batch."""
+        return self._prove(list(traces), list(boundaries), transition_zerofier_codeword, proof_streams, seeds)
+
+    def _prove(self, traces, boundaries, transition_zerofier_codeword, proof_streams, seeds, columns=None):
+        """prove_batch, or with `columns` (traces None) the proofs of the traces already in that column buffer"""
         T, nregs = self.trace_length, self.nregs
         where = self._where()
 
@@ -552,7 +570,7 @@ class StarkPlan(_Stages):
                 return [(quots[where[k.index][0]][b, where[k.index][1], :k.bound + 1], k.bound) for k in self.cons]
             return rows_of, degree_check
 
-        streams, quadrupled = self._prove_batch(list(traces), list(boundaries), proof_streams, transition, seeds)
+        streams, quadrupled = self._prove_batch(traces, boundaries, proof_streams, transition, seeds, columns)
 
         # ... and the zerofier's openings (:171-175), proof by proof: the codeword is the caller's
         zc = transition_zerofier_codeword
@@ -649,6 +667,10 @@ class PlainStarkPlan(_Stages):
         gives from the same draws (DESIGN section 3.11).  The exception is the one proving the proofs one at a time
         in order raises first, with the failing proof's index as ``proof_index``.  `seeds` as
         StarkPlan.prove_batch's."""
+        return self._prove(list(traces), list(boundaries), proof_streams, seeds)
+
+    def _prove(self, traces, boundaries, proof_streams, seeds, columns=None):
+        """prove_batch, or with `columns` (traces None) the proofs of the traces already in that column buffer"""
         T, nregs = self.trace_length, self.nregs
 
         def transition(eng, polys, failed, B):
@@ -696,7 +718,7 @@ class PlainStarkPlan(_Stages):
                 return rows
             return rows_of, degree_check
 
-        streams, _ = self._prove_batch(list(traces), list(boundaries), proof_streams, transition, seeds)
+        streams, _ = self._prove_batch(traces, boundaries, proof_streams, transition, seeds, columns)
         return [ps.serialize() for ps in streams]
 
 
@@ -731,6 +753,57 @@ def sign_batch(signer, sk, documents, seeds=None):
                                 signer.transition_zerofier_codeword, streams, seeds)
     plan = PlainStarkPlan(stark, transition)
     return plan.prove_batch([trace] * len(documents), [boundary] * len(documents), streams, seeds)
+
+
+class SignerPlan:
+    """What does not change between signatures of an RPSSS or FastRPSSS instance `signer`: its transition
+    constraints (rp.transition_constraints, built once), the PlainStarkPlan for a Stark or the StarkPlan with the
+    signer's zerofier for a FastStark, and the device copy of its Rescue constants (sa_rescue).  ``sign`` signs any
+    number of (key, document) pairs per call, and a plan serves any number of calls (DESIGN section 3.14)."""
+
+    def __init__(self, signer):
+        import sys
+        rp, stark = signer.rp, signer.stark
+        assert stark.original_trace_length == rp.N + 1 and stark.num_registers == 2, \
+            "sa_stark: the signer's Stark proves %d cycles of %d registers, not the %d rows of 2 of its Rescue trace" \
+            % (stark.original_trace_length, stark.num_registers, rp.N + 1)
+        self.rp, self.stark = rp, stark
+        self.constants = sa_rescue.upload_constants(sa_engine.get_engine(), rp)
+        transition = rp.transition_constraints(stark.omicron)
+        if hasattr(signer, "transition_zerofier"):
+            self.plan = StarkPlan(stark, transition, signer.transition_zerofier)
+            self.zerofier_codeword = signer.transition_zerofier_codeword
+        else:
+            self.plan = PlainStarkPlan(stark, transition)
+            self.zerofier_codeword = None
+        self.stream = sys.modules[type(signer).__module__].SignatureProofStream
+
+    def sign(self, sks, documents, seeds=None):
+        """[signer.sign(sks[d], documents[d]) for each d]: one sa_rescue launch writes every key's trace into rows
+        0 .. N of the prover's column buffer, the public keys are read from row N of register 0 with one gather, and
+        the batch is proven as prove_batch proves it, each document with its own SignatureProofStream.  No trace
+        element crosses to the device.  Unseeded, the draws are taken in prove_batch's order; with `seeds`, one
+        secret 32-byte seed per signature, signature d is signer.sign(sks[d], documents[d]) with os.urandom =
+        seeded_urandom(seeds[d]), whatever the batch.  Unequal lengths, bad seeds and keys that are not elements of p
+        raise an AssertionError before any device work."""
+        sks, documents = list(sks), list(documents)
+        assert len(sks) == len(documents), "sa_stark: %d keys and %d documents" % (len(sks), len(documents))
+        seeds = _seeds(seeds, len(documents))
+        keys = sa_rescue.values(sks, "secret key")
+        if not keys:
+            return []
+        eng = sa_engine.get_engine()
+        rp, plan, B, N, T = self.rp, self.plan, len(keys), self.rp.N, self.plan.trace_length
+        columns = eng.empty(B * 2 * T).reshape(B * 2, T, 2)
+        eng.rescue(eng.upload(sa_devlist.pack(keys)), self.constants, N, rp.alpha, rp.alphainv, trace=columns,
+                   inst_stride=2 * T, lane_stride=T)
+        pks = eng.gather_batch(columns.reshape(1, B * 2 * T, 2), [b * 2 * T + N for b in range(B)])
+        element = type(rp.round_constants[0])
+        boundaries = [rp.boundary_constraints(element(_value(lo, hi), rp.field)) for lo, hi in pks.reshape(B, 2)]
+        streams = [self.stream(d) for d in documents]
+        if self.zerofier_codeword is not None:
+            return plan._prove(None, boundaries, self.zerofier_codeword, streams, seeds, columns)
+        return plan._prove(None, boundaries, streams, seeds, columns)
 
 
 _originals = {}  # class -> its own `prove` attribute before enable (None: inherited)
