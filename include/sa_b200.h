@@ -518,10 +518,17 @@ int sa_release_workspaces(void);
  * `count` pseudo-random pairs (plus edge cases) on the device; returns the number of
  * mismatches (0 = pass) or a negative SA_E* code.                                         */
 long long sa_selftest_field(size_t count, uint64_t seed);
+/* The same for the NTT tile's own product and butterfly (tile_mul, tile_bfly): npairs operand
+ * pairs (x, w) from the caller, each element two little-endian 64-bit words below p (pairs[4k..4k+1]
+ * = x, pairs[4k+2..4k+3] = w), then `count` pseudo-random and edge pairs; the butterfly's other
+ * operand is drawn.  Returns the number of mismatches, SA_ESIZE for a missing list or an element
+ * not below p, or a negative SA_E* code.                                                  */
+long long sa_selftest_tile(size_t count, uint64_t seed, const uint64_t *pairs, size_t npairs);
 /* Micro-benchmark: n_threads threads each run `iters` dependent rounds of `ilp`
  * independent operations of kind op (0 montmul, 1 add, 2 sub, 3 butterfly; 4 = blake2b node
- * compressions, 256 threads per block whatever `threads` says, ilp 1 or 2).  Returns the
- * kernel time in milliseconds (negative on error).                                        */
+ * compressions, 256 threads per block whatever `threads` says, ilp 1 or 2; 5 = op 3 through
+ * the NTT tile's butterfly tile_bfly).  Returns the kernel time in milliseconds (negative on
+ * error).                                                                                  */
 double sa_microbench(int op, int ilp, int iters, int blocks, int threads);
 
 #ifdef __cplusplus

@@ -111,6 +111,115 @@ SA_HDC int tile_bitrev(int i, int r) {
     return j;
 }
 
+// ---- the tile's own field product and butterfly.  Same canonical residues as fe_montmul / fe_add /
+// fe_sub; the device bodies are written for the tile kernels' instruction mix (field.cuh stays what every
+// other kernel compiles), the host and SA_PORTABLE_FIELD bodies are the portable field.
+#if defined(__CUDA_ARCH__) && !defined(SA_PORTABLE_FIELD)
+// Montgomery product x * w * 2^-128 mod p, the reduction of fe_montmul (field.cuh).  Every multiply-add
+// is one IMAD.WIDE whose 64-bit accumulator is an aligned register pair from start to end:
+//  * the schoolbook sums the products with i+j even into pairs (0,1) (2,3) (4,5) (6,7) and the odd ones
+//    into (1,2) (3,4) (5,6).  A chain either ends in a pair it initialises (a*b + carry, no addend) or
+//    leaves its carry in a register; the three such carries (word 5, 6, 7) are the addend of pair (5,6)
+//    and the word-7 term of the final merge t = even + odd, so no pair is built from a copy or a zero.
+//  * the reduction's four products t0 P3, t1 P3, t2 P3, m3 P3 are plain 64-bit products (no addend), merged
+//    by one add chain into u = m P3 >> 32.  The borrow w of m3 = t3 - x is taken again as the borrow-in of
+//    r = t_hi - u - w: a carry chain never consumes a borrow (that mix computed wrong results on the device).
+//  Rows of the product as 32-bit halves (mul.lo + mul.hi) become IMAD + IMAD.HI, and IMAD.HI costs as much
+//  as IMAD.WIDE (tools/pipebench.cu), so the first row and the reduction use mul.wide.  The add-back of p
+//  keeps its mask words on the multiplier pipe: the ALU pipe is the busier one once the copies are gone.
+__device__ __forceinline__ fe tile_mul(const fe &x, const fe &w) {
+    uint32_t t0, t1, t2, t3, t4, t5, t6, t7;
+    asm("{\n\t"
+        ".reg .u32 e1, e2, e3, e4, e5, e6, e7, o1, o2, o3, o4, o5, o6, k5, k6, k7;\n\t"
+        ".reg .u64 E0, E2, O1, O3;\n\t"
+        "mul.wide.u32 E0, %8, %12;\n\t"  // (0,0)@0 -> (t0, e1)
+        "mul.wide.u32 E2, %8, %14;\n\t"  // (0,2)@2
+        "mul.wide.u32 O1, %8, %13;\n\t"  // (0,1)@1
+        "mul.wide.u32 O3, %8, %15;\n\t"  // (0,3)@3
+        "mov.b64 {%0, e1}, E0;\n\t"
+        "mov.b64 {e2, e3}, E2;\n\t"
+        "mov.b64 {o1, o2}, O1;\n\t"
+        "mov.b64 {o3, o4}, O3;\n\t"
+        "mad.lo.cc.u32 e2, %9, %13, e2;\n\t"  // (1,1)@2, then (1,3) initialises (4,5)
+        "madc.hi.cc.u32 e3, %9, %13, e3;\n\t"
+        "madc.lo.cc.u32 e4, %9, %15, 0;\n\t"
+        "madc.hi.u32 e5, %9, %15, 0;\n\t"
+        "mad.lo.cc.u32 e4, %11, %13, e4;\n\t"  // (3,1)@4 -> carry k6
+        "madc.hi.cc.u32 e5, %11, %13, e5;\n\t"
+        "addc.u32 k6, 0, 0;\n\t"
+        "mad.lo.cc.u32 o3, %10, %13, o3;\n\t"  // (2,1)@3 -> carry k5
+        "madc.hi.cc.u32 o4, %10, %13, o4;\n\t"
+        "addc.u32 k5, 0, 0;\n\t"
+        "mad.lo.cc.u32 o1, %9, %12, o1;\n\t"  // (1,0)@1 (1,2)@3, then (2,3) + (k5, k6) initialises (5,6)
+        "madc.hi.cc.u32 o2, %9, %12, o2;\n\t"
+        "madc.lo.cc.u32 o3, %9, %14, o3;\n\t"
+        "madc.hi.cc.u32 o4, %9, %14, o4;\n\t"
+        "madc.lo.cc.u32 o5, %10, %15, k5;\n\t"
+        "madc.hi.u32 o6, %10, %15, k6;\n\t"
+        "mad.lo.cc.u32 o3, %11, %12, o3;\n\t"  // (3,0)@3 (3,2)@5 -> carry k7
+        "madc.hi.cc.u32 o4, %11, %12, o4;\n\t"
+        "madc.lo.cc.u32 o5, %11, %14, o5;\n\t"
+        "madc.hi.cc.u32 o6, %11, %14, o6;\n\t"
+        "addc.u32 k7, 0, 0;\n\t"
+        "mad.lo.cc.u32 e2, %10, %12, e2;\n\t"  // (2,0)@2 (2,2)@4, then (3,3) initialises (6,7)
+        "madc.hi.cc.u32 e3, %10, %12, e3;\n\t"
+        "madc.lo.cc.u32 e4, %10, %14, e4;\n\t"
+        "madc.hi.cc.u32 e5, %10, %14, e5;\n\t"
+        "madc.lo.cc.u32 e6, %11, %15, 0;\n\t"
+        "madc.hi.u32 e7, %11, %15, 0;\n\t"
+        "add.cc.u32 %1, e1, o1;\n\t"  // t = even + (odd << 32) + (k7 << 224)
+        "addc.cc.u32 %2, e2, o2;\n\t"
+        "addc.cc.u32 %3, e3, o3;\n\t"
+        "addc.cc.u32 %4, e4, o4;\n\t"
+        "addc.cc.u32 %5, e5, o5;\n\t"
+        "addc.cc.u32 %6, e6, o6;\n\t"
+        "addc.u32 %7, e7, k7;\n\t"
+        "}"
+        : "=r"(t0), "=r"(t1), "=r"(t2), "=r"(t3), "=r"(t4), "=r"(t5), "=r"(t6), "=r"(t7)
+        : "r"(x.v[0]), "r"(x.v[1]), "r"(x.v[2]), "r"(x.v[3]), "r"(w.v[0]), "r"(w.v[1]), "r"(w.v[2]), "r"(w.v[3]));
+    uint32_t r0, r1, r2, r3, top;
+    asm("{\n\t"
+        ".reg .u32 x, m3, h0, q1, q2, g2, g3, v3, v4, u1, u2, u3, u4;\n\t"
+        ".reg .u64 T, Q, G, V;\n\t"
+        "mul.wide.u32 T, %5, 0xCB800000;\n\t"  // (x, h0) = t0 P3: x = t0 P3 mod 2^32
+        "mul.wide.u32 Q, %6, 0xCB800000;\n\t"
+        "mul.wide.u32 G, %7, 0xCB800000;\n\t"
+        "mov.b64 {x, h0}, T;\n\t"
+        "mov.b64 {q1, q2}, Q;\n\t"
+        "mov.b64 {g2, g3}, G;\n\t"
+        "sub.u32 m3, %8, x;\n\t"  // m3 = t3 - x mod 2^32
+        "mul.wide.u32 V, m3, 0xCB800000;\n\t"
+        "mov.b64 {v3, v4}, V;\n\t"
+        "add.cc.u32 u1, h0, q1;\n\t"  // u = m P3 >> 32
+        "addc.cc.u32 u2, q2, g2;\n\t"
+        "addc.cc.u32 u3, g3, v3;\n\t"
+        "addc.u32 u4, v4, 0;\n\t"
+        "sub.cc.u32 x, %8, x;\n\t"  // the borrow w of t3 - x starts r = t_hi - u - w, in (-p, p)
+        "subc.cc.u32 %0, %9, u1;\n\t"
+        "subc.cc.u32 %1, %10, u2;\n\t"
+        "subc.cc.u32 %2, %11, u3;\n\t"
+        "subc.cc.u32 %3, %12, u4;\n\t"
+        "subc.u32 %4, 0, 0;\n\t"
+        "}"
+        : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3), "=r"(top)
+        : "r"(t0), "r"(t1), "r"(t2), "r"(t3), "r"(t4), "r"(t5), "r"(t6), "r"(t7));
+    return fe_cond_add_p<false>(r0, r1, r2, r3, top);
+}
+// (e, x) -> (e + x w, e - x w)
+__device__ __forceinline__ void tile_bfly(fe &e, fe &x, const fe &w) {
+    const fe t = tile_mul(x, w);
+    x = fe_sub(e, t);
+    e = fe_add(e, t);
+}
+#else
+SA_HD fe tile_mul(const fe &x, const fe &w) { return fe_montmul_portable(x, w); }
+SA_HD void tile_bfly(fe &e, fe &x, const fe &w) {
+    const fe t = fe_montmul_portable(x, w);
+    x = fe_sub_portable(e, t);
+    e = fe_add_portable(e, t);
+}
+#endif
+
 // one radix-2 decimation-in-time level (span LEN) of an R-point transform held in registers
 template <int R, int LEN>
 SA_HD void dft_level(fe *x, const fe *cst, int cstep) {
@@ -123,10 +232,13 @@ SA_HD void dft_level(fe *x, const fe *cst, int cstep) {
 #pragma unroll
 #endif
         for (int k = 0; k < HALF; k++) {
-            const fe t = (k == 0) ? x[g + k + HALF] : fe_montmul(x[g + k + HALF], cst[k * STEP * cstep]);
-            const fe e = x[g + k];
-            x[g + k] = fe_add(e, t);
-            x[g + k + HALF] = fe_sub(e, t);
+            if (k == 0) {
+                const fe e = x[g], t = x[g + HALF];
+                x[g] = fe_add(e, t);
+                x[g + HALF] = fe_sub(e, t);
+            } else {
+                tile_bfly(x[g + k], x[g + k + HALF], cst[k * STEP * cstep]);
+            }
         }
     }
     if constexpr (LEN < R) dft_level<R, LEN * 2>(x, cst, cstep);
@@ -286,7 +398,7 @@ SA_HD void ntt_tile_full_stage(int t, fe *sm, const TileArgs &a, long long b, in
 #endif
     for (int k = 1; k < R; k++) {
         const fe w = tile_ld(tw + tile_tw_slot((k * m) << wlog));
-        tile_st(sm + (row0 + k * M) * C + c, fe_montmul(x[k], w));
+        tile_st(sm + (row0 + k * M) * C + c, tile_mul(x[k], w));
     }
 }
 
@@ -340,11 +452,11 @@ SA_HD void ntt_tile_last_stage(int t, fe *sm, const TileArgs &a, long long b, in
             const unsigned o = (unsigned)tile_digit_reverse<LOGL, ELOG, C>(row0 + k);
             fe v = x[k];
             if constexpr (TWB2) {
-                if (active) v = fe_montmul(fe_montmul(v, tile_ldg(twb_a + o * twb_sr)), tile_ldg(twb_b + o * twb_b_sr));
+                if (active) v = tile_mul(tile_mul(v, tile_ldg(twb_a + o * twb_sr)), tile_ldg(twb_b + o * twb_b_sr));
             } else if (use_twb && active) {
-                v = fe_montmul(v, tile_ldg(twb + o * twb_sr));
+                v = tile_mul(v, tile_ldg(twb + o * twb_sr));
             }
-            if (use_scale) v = fe_montmul(v, a.scale);
+            if (use_scale) v = tile_mul(v, a.scale);
             if (active) {
                 if constexpr ((FLAGS & TF_PEERS) != 0) {
                     const long long rel = (dst - a.out) + (long long)(o * out_sr);

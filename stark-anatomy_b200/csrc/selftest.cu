@@ -1,5 +1,5 @@
-// selftest.cu -- the field self test (PTX carry chains against the portable C++ arithmetic) and the
-// microbenchmarks of the field product and the blake2b compression.
+// selftest.cu -- the field self tests (PTX carry chains of field.cuh and of the NTT tile's butterfly against
+// the portable C++ arithmetic) and the microbenchmarks of the field product and the blake2b compression.
 #include "fri_merkle.cuh"
 #include "ntt_tile.cuh"
 #include "runtime.cuh"
@@ -42,6 +42,32 @@ __global__ void k_selftest_field(unsigned long long *mismatches, long long count
     if (bad) atomicAdd(mismatches, (unsigned long long)bad);
 }
 
+// tile_mul / tile_bfly (ntt_tile.cuh) against the portable field: item i < npairs takes (x, w) from the
+// caller's list, the others draw random and edge operands; the butterfly's e is always drawn
+__global__ void k_selftest_tile(unsigned long long *mismatches, long long count, uint64_t seed, const fe *pairs,
+                                long long npairs) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count + npairs) return;
+    uint64_t s = seed + 0x9E3779B1ULL * (uint64_t)i;
+    const fe e = sa_rand_fe(s, (int)(i % 43));
+    fe x, w;
+    if (i < npairs) {
+        x = pairs[2 * i];
+        w = pairs[2 * i + 1];
+    } else {
+        x = sa_rand_fe(s, (int)(i % 37));
+        w = sa_rand_fe(s, (int)((i / 37) % 41));
+    }
+    const fe t = fe_montmul_portable(x, w);
+    fe lo = e, hi = x;
+    tile_bfly(lo, hi, w);
+    int bad = 0;
+    bad += !fe_eq(tile_mul(x, w), t);
+    bad += !fe_eq(lo, fe_add_portable(e, t));
+    bad += !fe_eq(hi, fe_sub_portable(e, t));
+    if (bad) atomicAdd(mismatches, (unsigned long long)bad);
+}
+
 template <int OP, int ILP>
 __global__ void k_microbench(fe *sink, int iters) {
     fe x[ILP], y[ILP];
@@ -63,6 +89,10 @@ __global__ void k_microbench(fe *sink, int iters) {
                 x[i] = fe_add(e, tt);
                 y[i] = fe_sub(e, tt);
             }
+            if (OP == 5) {  // op 3 through the NTT tile's butterfly
+                const fe w = x[(i + 1) % ILP];
+                tile_bfly(x[i], y[i], w);
+            }
         }
     }
     fe acc = x[0];
@@ -81,6 +111,36 @@ long long sa_selftest_field(size_t count, uint64_t seed) {
     SA_LAUNCH_CHECK();
     SA_CUDA(cudaMemcpy(&h, d, 8, cudaMemcpyDeviceToHost));
     cudaFree(d);
+    return (long long)h;
+}
+
+long long sa_selftest_tile(size_t count, uint64_t seed, const uint64_t *pairs, size_t npairs) {
+    if (npairs > 0 && pairs == nullptr) return SA_ESIZE;
+    for (size_t k = 0; k < 2 * npairs; k++) {  // the pairs are field elements: canonical, below p
+        const uint64_t hi = pairs[2 * k + 1];
+        if (hi > ((uint64_t)P3 << 32) || (hi == ((uint64_t)P3 << 32) && pairs[2 * k] != 0)) return SA_ESIZE;
+    }
+    // one allocation: the mismatch counter, then the pairs as 16-byte elements
+    char *d = nullptr;
+    unsigned long long h = 0;
+    SA_CUDA(cudaMalloc(&d, sizeof(fe) * (1 + 2 * npairs)));
+    const fe *dp = reinterpret_cast<const fe *>(d) + 1;
+    cudaError_t e = cudaMemset(d, 0, 8);
+    if (e == cudaSuccess && npairs > 0)
+        e = cudaMemcpy((void *)dp, pairs, sizeof(fe) * 2 * npairs, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(d);
+        SA_CUDA(e);
+    }
+    const long long total = (long long)(count + npairs);
+    if (total > 0)
+        k_selftest_tile<<<(unsigned)((total + 255) / 256), 256>>>(reinterpret_cast<unsigned long long *>(d),
+                                                                  (long long)count, seed, dp, (long long)npairs);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpy(&h, d, 8, cudaMemcpyDeviceToHost);
+    cudaFree(d);
+    SA_CUDA(e);
+    if (total > 0) g_launches.fetch_add(1, std::memory_order_relaxed);
     return (long long)h;
 }
 
@@ -121,6 +181,7 @@ double sa_microbench(int op, int ilp, int iters, int blocks, int threads) {
         case 2: ms = microbench_op<2>(ilp, iters, blocks, threads, sink); break;
         case 3: ms = microbench_op<3>(ilp, iters, blocks, threads, sink); break;
         case 4: ms = microbench_b2_ms(ilp, iters, blocks, (uint64_t *)sink); break;  // (merkle_fri.cu)
+        case 5: ms = microbench_op<5>(ilp, iters, blocks, threads, sink); break;
     }
     g_launches.fetch_add(2);
     if (cudaGetLastError() != cudaSuccess) ms = -1.0;

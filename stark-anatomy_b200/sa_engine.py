@@ -105,6 +105,7 @@ SYMBOLS = [
     ("sa_cache_bytes", _sz, []),
     ("sa_release_workspaces", _ci, []),
     ("sa_selftest_field", ctypes.c_longlong, [_sz, ctypes.c_uint64]),
+    ("sa_selftest_tile", ctypes.c_longlong, [_sz, ctypes.c_uint64, _u64p, _sz]),
     ("sa_microbench", ctypes.c_double, [_ci, _ci, _ci, _ci, _ci]),
 ]
 

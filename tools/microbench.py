@@ -9,9 +9,9 @@ lib = sa_engine.load_library()
 import torch
 torch.cuda.init()
 sm_count = torch.cuda.get_device_properties(0).multi_processor_count
-names = {0: "montmul", 1: "add", 2: "sub", 3: "butterfly"}
+names = {0: "montmul", 1: "add", 2: "sub", 3: "butterfly", 5: "tile butterfly"}
 iters, blocks, threads = 2000, sm_count * 4, 256
-for op in (0, 1, 2, 3):
+for op in (0, 1, 2, 3, 5):
     for ilp in (1, 2, 4, 8):
         ms = lib.sa_microbench(op, ilp, iters, blocks, threads)
         ops = iters * ilp * blocks * threads
