@@ -513,6 +513,49 @@ size_t sa_cache_limit(size_t bytes);
 size_t sa_cache_bytes(void);
 int sa_release_workspaces(void);
 
+/* ---- batched verification (code/fast_stark.py:180-286, code/stark.py:172-275, code/fri.py:132-231) -----------
+ * DESIGN section 3.15.  Every call writes one flag per item, 0 where the item's check passes; items are independent,
+ * one thread each, in one grid-stride launch.  count == 0 returns SA_OK without a launch.  Before any launch: SA_ESIZE
+ * for an item count (or a largest element offset the sizes imply) at or above 2^59 and for a NULL buffer.  No
+ * allocation; asynchronous and graph-capturable.
+ *
+ * sa_merkle_verify_batch: Merkle.verify(root, index, path, leaf) for path i: blake2b of leaves[i]'s decimal ASCII,
+ * then depth[i] levels bottom-up, level l hashing (cur || sibling) when bit l of leaf_index[i] is 0 and (sibling ||
+ * cur) when it is 1, the last digest compared with the 64 bytes at roots + 64 i.  Sibling l of path i is the 64
+ * bytes at paths + 64 (path_offset[i] + l): paths of different depths share one launch.  An index at or above
+ * 2^depth[i] or a depth above 63 is a failed check.                                                              */
+int sa_merkle_verify_batch(uint32_t *flags, const void *roots, const void *leaves, const uint64_t *leaf_index,
+                           const uint32_t *depth, const void *paths, const uint64_t *path_offset, size_t count,
+                           void *stream);
+/* sa_fri_colinear_batch: FRI's colinearity test for item i of round r = round[i] at a-index a = a_index[i]:
+ * test_colinearity([(ax, ay[i]), (-ax, by[i]), (alpha[i], cy[i])]) with ax = offset^(2^r) omega^(2^r a), computed
+ * as the reference's Lagrange interpolant (inverse(0) = 0) having degree exactly 1.                            */
+int sa_fri_colinear_batch(uint32_t *flags, const void *ay, const void *by, const void *cy, const uint64_t *a_index,
+                          const void *alpha, const uint32_t *round, const uint64_t offset[2], const uint64_t omega[2],
+                          size_t count, void *stream);
+/* sa_verify_combination: the verifier's combination at k opened indices of each of nproofs proofs, items and
+ * proofs laid out as csrc/verify.cuh states (verify_item, verify_proof): the trace values from each register's
+ * boundary zerofier and interpolant (blen coefficients each) by Horner, the AIR at [x, cur, next] by walking the
+ * program sa_air_program compiled (ncons constraints of nregs registers), the transition zerofier's value from the
+ * item (zcoef NULL) or by Horner over zcoef[0..zlen), and the weighted sum with x^shift, compared with FRI's value.
+ * x = offset omega^i on the domain of 2^log_n points, the next point at (i + ef) mod 2^log_n.  Flag 1 for a
+ * mismatch, 2 for a zero zerofier value.  SA_ESIZE also for nregs outside 1..16, ncons or blen outside 1..2^32 - 1,
+ * log_n outside 1..30, ef >= 2^log_n and zlen == 0 with zcoef.                                                  */
+int sa_verify_combination(uint32_t *flags, const void *items, const void *proofs, size_t k, size_t nproofs,
+                          const void *prog, size_t ncons, size_t nregs, size_t blen, const void *zcoef, size_t zlen,
+                          const uint64_t offset[2], const uint64_t omega[2], int log_n, size_t ef, void *stream);
+/* sa_poly_degree_batch: degrees[b] = the highest j < n with coeffs[b n + j] != 0, or -1 for a zero row (int64,
+ * device memory), for batch rows of n elements.  SA_ESIZE for n not a power of two in 1..2^30.  One memset and one
+ * launch.                                                                                                       */
+int sa_poly_degree_batch(long long *degrees, const void *coeffs, size_t n, size_t batch, void *stream);
+/* sa_air_program: the transition constraints (sa_air_plan's coeffs, exps, term_start, HOST arrays) compiled into
+ * the program sa_air_plan keeps in its plan, written to prog (device memory of sa_air_program_bytes(nterms, nregs)
+ * bytes, nterms = term_start[ncons] - term_start[0]; 0 for unsupported sizes).  Synchronises.  SA_ESIZE for ncons
+ * or nregs == 0 or a decreasing term_start.                                                                     */
+size_t sa_air_program_bytes(size_t nterms, size_t nregs);
+int sa_air_program(void *prog, const uint64_t *coeffs, const uint32_t *exps, const size_t *term_start, size_t ncons,
+                   size_t nregs, void *stream);
+
 /* ---- self checks (used by tests / smoke) ------------------------------------------------
  * Runs the device carry-chain field arithmetic against the portable C++ version on
  * `count` pseudo-random pairs (plus edge cases) on the device; returns the number of

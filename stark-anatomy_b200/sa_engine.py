@@ -98,6 +98,13 @@ SYMBOLS = [
     ("sa_gather_batch_sets", _ci, [_vp, _vp, _sz, _sz, _sz, _u64p, _sz, _vp]),
     ("sa_sample_seeded", _ci, [_vp, _vp, _sz, _sz, ctypes.c_uint64, _sz, _sz, _sz, _vp]),
     ("sa_rescue", _ci, [_vp, _vp, _vp, _sz, _vp, _sz, _u64p, _u64p, _sz, _sz, _vp]),
+    ("sa_merkle_verify_batch", _ci, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    ("sa_fri_colinear_batch", _ci, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _u64p, _u64p, _sz, _vp]),
+    ("sa_verify_combination", _ci, [_vp, _vp, _vp, _sz, _sz, _vp, _sz, _sz, _sz, _vp, _sz, _u64p, _u64p, _ci, _sz,
+                                    _vp]),
+    ("sa_poly_degree_batch", _ci, [_vp, _vp, _sz, _sz, _vp]),
+    ("sa_air_program_bytes", _sz, [_sz, _sz]),
+    ("sa_air_program", _ci, [_vp, _u64p, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(_sz), _sz, _sz, _vp]),
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_commit", _ci, [_vp, _vp, _vp, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
@@ -916,6 +923,73 @@ class CudaEngine:
                                        constants.data_ptr(), rounds, _limbs(alpha), _limbs(alphainv), inst_stride,
                                        lane_stride, self._stream()))
         return hashes, trace
+
+    # --------------------------------------------------------------- verify
+    def air_program(self, constraints, nregs):
+        """sa_air_program: the transition constraints (as air_plan takes them) compiled into the program the
+        combination walks, a uint8 device tensor (synchronises)"""
+        nregs, constraints = int(nregs), list(constraints)
+        if nregs < 1 or not constraints:
+            raise SaError(SA_ERRORS[-6])
+        coeffs, exps, starts = _air_arrays(constraints, nregs)
+        nbytes = self.lib.sa_air_program_bytes(starts[-1], nregs)
+        if nbytes == 0:
+            raise SaError(SA_ERRORS[-6])
+        prog = self.torch.empty(nbytes, dtype=self.torch.uint8, device=self.device)
+        ncons = len(constraints)
+        self._check(self.lib.sa_air_program(
+            prog.data_ptr(), (ctypes.c_uint64 * max(len(coeffs), 1))(*coeffs),
+            (ctypes.c_uint32 * max(len(exps), 1))(*exps), (ctypes.c_size_t * (ncons + 1))(*starts), ncons, nregs,
+            self._stream()))
+        return prog
+
+    def upload_bytes(self, buf):
+        """a host bytes-like object -> one uint8 device tensor (one upload)"""
+        torch = self.torch
+        host = torch.frombuffer(bytearray(buf), dtype=torch.uint8) if len(buf) else torch.empty(0, dtype=torch.uint8)
+        self._count("h2d", host.numel())
+        return host.to(self.device)
+
+    def verify_chunk(self, buf, L):
+        """The device checks of one chunk of proofs (DESIGN section 3.15) from `buf`, the chunk's one uploaded uint8
+        tensor, whose sections start at the byte offsets of the layout L (sa_stark.VerifierPlan._pack):
+        sa_merkle_verify_batch over L["paths"] paths, sa_fri_colinear_batch over L["colinear"] items,
+        sa_verify_combination over L["k"] indices of L["proofs"] proofs, and for the proofs' last codewords one
+        sa_merkle_tree_batch, one batched inverse sa_ntt and sa_poly_degree_batch.  Everything lands in one result
+        buffer read with one download: (Merkle flags, colinearity flags, combination flags, the last codewords'
+        degrees, their tree roots as bytes)."""
+        torch, st = self.torch, self._stream()
+        lib = self.lib
+        ptr = buf.data_ptr()
+        at = lambda name: ptr + L[name]  # noqa: E731
+        npath, ncol, B, k, m = L["paths"], L["colinear"], L["proofs"], L["k"], L["last_len"]
+        nflag = npath + ncol + B * k
+        res = torch.empty(4 * nflag + 8 * B + 64 * B + 8, dtype=torch.uint8, device=self.device)
+        flags = res.data_ptr()
+        deg_at = 4 * nflag + (-4 * nflag) % 8
+        self._check(lib.sa_merkle_verify_batch(flags, at("roots"), at("leaves"), at("leaf_index"), at("depth"),
+                                               at("digests"), at("path_offset"), npath, st))
+        self._check(lib.sa_fri_colinear_batch(flags + 4 * npath, at("ay"), at("by"), at("cy"), at("a_index"),
+                                              at("alpha"), at("round"), _limbs(L["fri_offset"]),
+                                              _limbs(L["fri_omega"]), ncol, st))
+        zcoef = L.get("zcoef")
+        self._check(lib.sa_verify_combination(flags + 4 * (npath + ncol), at("items"), at("proof_data"), k, B,
+                                              L["prog"].data_ptr(), L["ncons"], L["nregs"], L["blen"],
+                                              None if zcoef is None else zcoef.data_ptr(),
+                                              0 if zcoef is None else zcoef.shape[0], _limbs(L["offset"]),
+                                              _limbs(L["omega"]), L["log_n"], L["ef"], st))
+        if B:
+            last = buf[L["last"]:L["last"] + 16 * B * m].view(torch.int64).reshape(B, m, 2)
+            trees = self.merkle_trees(last)
+            coeffs = self.ntt(last.reshape(B * m, 2), m.bit_length() - 1, L["last_omega"], inverse=True, batch=B)
+            self._check(lib.sa_poly_degree_batch(flags + deg_at, coeffs.data_ptr(), m, B, st))
+            res[deg_at + 8 * B:deg_at + 72 * B].view(B, 64).copy_(trees[:, 1])
+        host = res.cpu().numpy()
+        self._count("d2h", res.numel())
+        import numpy as np
+        return (host[:4 * npath].view(np.uint32), host[4 * npath:4 * (npath + ncol)].view(np.uint32),
+                host[4 * (npath + ncol):4 * nflag].view(np.uint32), host[deg_at:deg_at + 8 * B].view(np.int64),
+                host[deg_at + 8 * B:deg_at + 72 * B].tobytes())
 
     # ------------------------------------------------------------------ fri
     def fri_fold(self, vec, alpha, offset, omega):

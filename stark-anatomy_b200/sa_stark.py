@@ -770,13 +770,16 @@ class SignerPlan:
         self.rp, self.stark = rp, stark
         self.constants = sa_rescue.upload_constants(sa_engine.get_engine(), rp)
         transition = rp.transition_constraints(stark.omicron)
+        self.transition = transition
         if hasattr(signer, "transition_zerofier"):
             self.plan = StarkPlan(stark, transition, signer.transition_zerofier)
             self.zerofier_codeword = signer.transition_zerofier_codeword
+            self.zerofier_root = getattr(signer, "transition_zerofier_root", None)
         else:
             self.plan = PlainStarkPlan(stark, transition)
-            self.zerofier_codeword = None
+            self.zerofier_codeword = self.zerofier_root = None
         self.stream = sys.modules[type(signer).__module__].SignatureProofStream
+        self._verifier = None
 
     def sign(self, sks, documents, seeds=None):
         """[signer.sign(sks[d], documents[d]) for each d]: one sa_rescue launch writes every key's trace into rows
@@ -806,7 +809,408 @@ class SignerPlan:
         return plan._prove(None, boundaries, streams, seeds, columns)
 
 
+    def verify(self, pks, documents, signatures, reasons=False):
+        """[signer.verify(pks[d], documents[d], signatures[d]) for each d] in one VerifierPlan.verify_batch call: the
+        boundary of rp.boundary_constraints(pk) and each document's SignatureProofStream, the verifier plan built on
+        the first call and kept"""
+        pks, documents, signatures = list(pks), list(documents), list(signatures)
+        assert len(pks) == len(documents) == len(signatures), \
+            "sa_stark: %d keys, %d documents and %d signatures" % (len(pks), len(documents), len(signatures))
+        assert self.zerofier_codeword is None or self.zerofier_root is not None, \
+            "sa_stark: the FastStark signer has no transition_zerofier_root to verify against"
+        if self._verifier is None:
+            self._verifier = VerifierPlan(self.stark, self.transition, self.zerofier_root)
+        return self._verifier.verify_batch(signatures, [self.rp.boundary_constraints(pk) for pk in pks],
+                                           [self.stream(d) for d in documents], reasons)
+
+
+# ---- verification (DESIGN section 3.15) ----
+FRI_MESSAGES = {"a": "merkle authentication path verification fails for aa",     # fri.py:214-224
+                "b": "merkle authentication path verification fails for bb",
+                "c": "merkle authentication path verification fails for cc"}
+LAST_FORM = "last codeword is not well formed"                                     # fri.py:148
+COLINEAR = "colinearity check failure"                                             # fri.py:208
+MALFORMED = "malformed"
+CHUNK_BYTES = 1 << 30  # one chunk's device buffers, as coset_batch_max bounds a coset call's
+
+
+def _xor_exponent(e):
+    """the exponent FieldElement.__xor__ (algebra.py:38-45) applies for an int e: e itself from 0 on; for a negative
+    e its bits over len(bin(e)) - 2 positions of the two's complement"""
+    return e if e >= 0 else e & ((1 << (len(bin(e)) - 2)) - 1)
+
+
+def _lagrange(xs, ys):
+    """Polynomial.interpolate_domain's coefficients (univariate.py:107-120), low to high, with inverse(0) = 0"""
+    acc = [0] * len(xs)
+    for j, (xj, yj) in enumerate(zip(xs, ys)):
+        basis, den = [1], 1
+        for m, xm in enumerate(xs):
+            if m != j:
+                basis = [((basis[t - 1] if t else 0) - xm * (basis[t] if t < len(basis) else 0)) % P
+                         for t in range(len(basis) + 1)]
+                den = den * (xj - xm) % P
+        f = yj * pow(den, P - 2, P) % P
+        for t, b in enumerate(basis):
+            acc[t] = (acc[t] + f * b) % P
+    return acc
+
+
+def _is_element(v):
+    return type(v).__name__ == "FieldElement" and type(getattr(v, "value", None)) is int and 0 <= v.value < P
+
+
+def _is_digest(d):
+    return type(d) is bytes and len(d) == 64
+
+
+def _is_path(path, depth):
+    return type(path) is list and len(path) == depth and all(_is_digest(d) for d in path)
+
+
+class _Refused(AssertionError):
+    """a statement VerifierPlan does not take (DESIGN section 3.15); enable_verify hands it to the original verify"""
+
+
+class _Parsed:
+    """one proof's transcript: what the host reads and derives, and the device items it contributes"""
+    __slots__ = ("weights", "fri_roots", "alphas", "last", "top_indices", "top", "triples", "fri_paths", "opened",
+                 "statement")
+
+
+class VerifierPlan:
+    """What does not change between verifications of one AIR: the FRI parameters, the compiled AIR program, the
+    transition quotients' shifts and, for a plain Stark, its transition zerofier on the device.  With a
+    `transition_zerofier_root` the plan verifies FastStark proofs (FastStark.verify, fast_stark.py:180-286; `stark`
+    a FastStark or a ``Params``), without one plain ones (Stark.verify, stark.py:172-275), the zerofier of omicron^0
+    .. omicron^(ncycles - 2) built as PlainStarkPlan builds it.
+
+    A verdict is the reference's for every proof whose stream has the reference's shape: the number of objects the
+    verifier pulls, 64-byte ``bytes`` roots, a last codeword of FieldElements of the length FRI gives, 3-tuples of
+    elements for the FRI leaves, lists of 64-byte digests of the tree's depth for paths and elements for opened
+    leaves.  A proof outside that shape is False (reason "malformed").  Everything but unpickling, Fiat-Shamir (the
+    stream's own verifier_fiat_shamir), the weights and the index sampling runs on the device (DESIGN section
+    3.15)."""
+
+    def __init__(self, stark, transition_constraints, transition_zerofier_root=None):
+        eng = sa_engine.get_engine()
+        self.stark = stark
+        self.constraints = list(transition_constraints)
+        self.zerofier_root = transition_zerofier_root
+        self.nregs = stark.num_registers
+        fri = stark.fri
+        self.fri = fri
+        self.n = fri.domain_length
+        self.log_n = self.n.bit_length() - 1
+        self.ef = fri.expansion_factor
+        self.k = fri.num_colinearity_tests
+        self.rounds = fri.num_rounds()
+        self.last_len = self.n >> (self.rounds - 1)
+        if not 1 <= self.nregs <= 16:
+            raise _Refused("sa_stark: the verifier takes 1 to 16 registers, not %d" % self.nregs)
+        if 1 << self.log_n != self.n or not 1 <= self.log_n <= 30:
+            raise _Refused("sa_stark: a FRI domain of %d points" % self.n)
+        self.prog = eng.air_program(self.constraints, self.nregs)
+        self.max_degree = stark.max_degree(self.constraints)
+        self.tshifts = [_xor_exponent(self.max_degree - b)
+                        for b in stark.transition_quotient_degree_bounds(self.constraints)]
+        if not all(0 <= s < 1 << 32 for s in self.tshifts):
+            raise _Refused("sa_stark: a transition shift at or above 2^32")
+        self.zcoef = None
+        if transition_zerofier_root is None:
+            ncycles = stark.original_trace_length
+            if ncycles < 2:
+                raise _Refused("sa_stark: a plain Stark of one cycle has no transition zerofier")
+            omicron = stark.omicron.value
+            if _tree_fits(eng, ncycles - 1):
+                points = [FieldElement(pow(omicron, i, P), stark.field) for i in range(ncycles - 1)]
+                self.zcoef = eng.zerofier(eng.upload(sa_devlist.pack(points)))
+            else:
+                self.zcoef = eng.geo_zerofier(omicron, ncycles - 1)
+        self._statements = {}
+
+    # -- the statement of one boundary: its zerofiers, interpolants and shifts (fast_stark.py:53-67, 272-277) --
+    def _statement(self, boundary):
+        key = tuple((int(c), int(r), int(getattr(v, "value", v))) for c, r, v in boundary)
+        st = self._statements.get(key)
+        if st is not None:
+            return st
+        stark, nregs = self.stark, self.nregs
+        rtl = 1 + max(c for c, _, _ in key) + stark.num_randomizers
+        omicron = stark.omicron.value
+        zs, its = [], []
+        for s in range(nregs):
+            pts = [(pow(omicron, c, P), v % P) for c, r, v in key if r == s]
+            if not pts:
+                raise AssertionError("cannot interpolate between zero points")  # univariate.py:109
+            z = [1]
+            for x, _ in pts:
+                z = [((z[t - 1] if t else 0) - x * (z[t] if t < len(z) else 0)) % P for t in range(len(z) + 1)]
+            zs.append(z)
+            its.append(_lagrange([x for x, _ in pts], [v for _, v in pts]))
+        bshifts = [_xor_exponent(self.max_degree - (rtl - 1 - (len(z) - 1))) for z in zs]
+        if not all(0 <= s < 1 << 32 for s in bshifts):
+            raise _Refused("sa_stark: a boundary shift at or above 2^32")
+        blen = max(len(z) for z in zs)
+        coef = []
+        for z, i in zip(zs, its):
+            coef += z + [0] * (blen - len(z)) + i + [0] * (blen - len(i))
+        st = (blen, self.tshifts + bshifts, coef)
+        self._statements[key] = st
+        return st
+
+    # -- one proof's transcript, in the reference's pull order; None outside the shape --
+    def _parse(self, proof, boundary, proof_stream):
+        stark, fri, nregs, k, rounds, n = self.stark, self.fri, self.nregs, self.k, self.rounds, self.n
+        max(c for c, _, _ in boundary)  # fast_stark.py:184: the trace length first (ValueError without points)
+        try:
+            ps = (proof_stream if proof_stream is not None else sa_host.ip.ProofStream()).deserialize(proof)
+        except Exception:
+            return None
+        objects = getattr(ps, "objects", None)
+        nopen = nregs + 1 + (self.zerofier_root is not None)
+        top = 2 * k if rounds > 1 else 0
+        count = nregs + 1 + rounds + 1 + (rounds - 1) * 4 * k + nopen * 2 * 2 * top
+        if type(objects) is not list or len(objects) < count:
+            return None
+        pr = _Parsed()
+        roots = [ps.pull() for _ in range(nregs + 1)]
+        # the boundary's interpolants and zerofiers after the roots' pulls (fast_stark.py:192-201), with their
+        # exceptions
+        pr.statement = self._statement(boundary)
+        if not all(_is_digest(r) for r in roots):
+            return None
+        W = 1 + 2 * len(self.constraints) + 2 * nregs
+        pr.weights = [w.value for w in stark.sample_weights(W, ps.verifier_fiat_shamir())]
+        pr.fri_roots, pr.alphas = [], []
+        for r in range(rounds):
+            pr.fri_roots.append(ps.pull())
+            pr.alphas.append(stark.field.sample(ps.verifier_fiat_shamir()).value)
+        if not all(_is_digest(r) for r in pr.fri_roots):
+            return None
+        last = ps.pull()
+        if type(last) is not list or len(last) != self.last_len or not all(_is_element(v) for v in last):
+            return None
+        pr.last = last
+        pr.top_indices = fri.sample_indices(ps.verifier_fiat_shamir(), n >> 1, n >> (rounds - 1), k) \
+            if rounds > 1 else []
+        pr.triples, pr.fri_paths = [], []
+        for r in range(rounds - 1):
+            triples = [ps.pull() for _ in range(k)]
+            if not all(type(t) is tuple and len(t) == 3 and all(_is_element(v) for v in t) for t in triples):
+                return None
+            paths = [ps.pull() for _ in range(3 * k)]
+            depth = self.log_n - r
+            if not all(_is_path(p, depth - (q % 3 == 2)) for q, p in enumerate(paths)):
+                return None
+            pr.triples.append(triples)
+            pr.fri_paths.append(paths)
+        # the combination's indices: FRI's round-0 a and b indices, sorted (fast_stark.py:205-211)
+        half = n >> 1
+        values = sorted([(i % half, pr.triples[0][s][0]) for s, i in enumerate(pr.top_indices)] +
+                        [(i % half + half, pr.triples[0][s][1]) for s, i in enumerate(pr.top_indices)],
+                        key=lambda iv: iv[0]) if top else []
+        dup = sorted([i for i, _ in values] + [(i + self.ef) % n for i, _ in values])
+        pr.opened = []  # (root, [(index, leaf, path)])
+        for root in roots + ([self.zerofier_root] if self.zerofier_root is not None else []):
+            reads = []
+            for i in dup:
+                leaf, path = ps.pull(), ps.pull()
+                if not _is_element(leaf) or not _is_path(path, self.log_n):
+                    return None
+                reads.append((i, leaf, path))
+            pr.opened.append((root, reads))
+        pr.top = values
+        return pr
+
+    # -- the packed buffer of a chunk: every section 16-byte aligned --
+    def _pack(self, parsed):
+        import numpy as np
+        nregs, k, rounds = self.nregs, self.k, self.rounds
+        roots, leaves, idx, depth, digests, poff = [], [], [], [], [], []
+        ay, by, cy, aidx, alpha, rnd = [], [], [], [], [], []
+        items, pdata, last = [], [], []
+        blen = max(pr.statement[0] for pr in parsed)
+        ncons = len(self.constraints)
+        ktop = len(parsed[0].top)
+
+        def path(root, i, leaf, p):
+            roots.append(root)
+            leaves.append(leaf)
+            idx.append(i)
+            depth.append(len(p))
+            poff.append(len(digests))
+            digests.extend(p)
+        for pr in parsed:
+            # FRI round r (fri.py:180-224): c = a = top index mod n / 2^(r+1), b = a + n / 2^(r+1); c opens in the
+            # next round's tree
+            for r in range(rounds - 1):
+                half = self.n >> (r + 1)
+                for s, t in enumerate(pr.triples[r]):
+                    a = pr.top_indices[s] % half
+                    ay.append(t[0])
+                    by.append(t[1])
+                    cy.append(t[2])
+                    aidx.append(a)
+                    alpha.append(pr.alphas[r])
+                    rnd.append(r)
+                for s, t in enumerate(pr.triples[r]):
+                    a = pr.top_indices[s] % half
+                    ps3 = pr.fri_paths[r][3 * s:3 * s + 3]
+                    path(pr.fri_roots[r], a, t[0], ps3[0])
+                    path(pr.fri_roots[r], a + half, t[1], ps3[1])
+                    path(pr.fri_roots[r + 1], a, t[2], ps3[2])
+            for root, reads in pr.opened:
+                for i, leaf, p in reads:
+                    path(root, i, leaf, p)
+            blen_p, shifts, coef = pr.statement
+            pdata += pr.weights + shifts
+            per = 2 * blen_p
+            for s in range(nregs):
+                z = coef[s * per:s * per + blen_p]
+                it = coef[s * per + blen_p:(s + 1) * per]
+                pdata += z + [0] * (blen - blen_p) + it + [0] * (blen - blen_p)
+            values = {}
+            for root_no, (root, reads) in enumerate(pr.opened):
+                for i, leaf, p in reads:
+                    values[(root_no, i)] = leaf  # a repeated index keeps the last leaf pulled, as the dict does
+            for i, v in pr.top:
+                j = (i + self.ef) % self.n
+                items += [i, v] + [values[(s, i)] for s in range(nregs)] + [values[(s, j)] for s in range(nregs)]
+                items += [values[(nregs, i)], values[(nregs + 1, i)] if self.zerofier_root is not None else 0]
+            last += pr.last
+        sections, L, size = [], {}, 0
+
+        def add(name, raw):
+            nonlocal size
+            raw = bytes(raw)
+            L[name] = size
+            pad = (-len(raw)) % 16
+            sections.append(raw + bytes(pad))
+            size += len(raw) + pad
+        add("roots", b"".join(roots))
+        add("leaves", sa_marshal.pack(leaves))
+        add("leaf_index", np.array(idx, dtype=np.uint64).tobytes())
+        add("depth", np.array(depth, dtype=np.uint32).tobytes())
+        add("digests", b"".join(digests))
+        add("path_offset", np.array(poff, dtype=np.uint64).tobytes())
+        for name, vals in (("ay", ay), ("by", by), ("cy", cy), ("alpha", alpha), ("items", items),
+                           ("proof_data", pdata), ("last", last)):
+            add(name, sa_marshal.pack(vals))
+        add("a_index", np.array(aidx, dtype=np.uint64).tobytes())
+        add("round", np.array(rnd, dtype=np.uint32).tobytes())
+        stark = self.stark
+        L.update(paths=len(idx), colinear=len(ay), proofs=len(parsed), k=ktop, last_len=self.last_len,
+                 fri_offset=self.fri.offset.value, fri_omega=self.fri.omega.value, prog=self.prog, ncons=ncons,
+                 nregs=nregs, blen=blen, offset=stark.generator.value, omega=stark.omega.value, log_n=self.log_n,
+                 ef=self.ef, zcoef=self.zcoef,
+                 last_omega=pow(self.fri.omega.value, 1 << (rounds - 1), P))
+        return b"".join(sections), L
+
+    def _decide(self, pr, mflags, cflags, kflags, degree, root):
+        """the reference's verdict from one proof's device flags, checks in the reference's order: (verdict, reason,
+        whether the zerofier vanished at the failing index)"""
+        k, rounds = self.k, self.rounds
+        if root != pr.fri_roots[-1]:
+            return False, LAST_FORM
+        bound = self.last_len // self.ef - 1
+        if degree > bound:
+            return False, ("last codeword does not correspond to polynomial of low enough degree\n"
+                           "observed degree: %d\nbut should be: %d" % (degree, bound))
+        m = 0
+        for r in range(rounds - 1):
+            for s in range(k):
+                if cflags[r * k + s]:
+                    return False, COLINEAR
+            for q in range(3 * k):
+                if mflags[m + q]:
+                    return False, FRI_MESSAGES["abc"[q % 3]]
+            m += 3 * k
+        if any(mflags[m:]):
+            return False, "leaf path"
+        for f in kflags:
+            if f == 2:
+                raise AssertionError("divide by zero")  # algebra.py:92
+            if f:
+                return False, "combination"
+        return True, None
+
+    def _bytes(self, pr):
+        """the device bytes one proof takes in a chunk: its packed sections, its flags and its last codeword's tree,
+        inverse transform, degree and root"""
+        npath = (self.rounds - 1) * 3 * self.k + sum(len(reads) for _, reads in pr.opened)
+        ndigest = sum(len(p) for paths in pr.fri_paths for p in paths) + sum(
+            len(p) for _, reads in pr.opened for _, _, p in reads)
+        ncol = (self.rounds - 1) * self.k
+        blen, shifts, _ = pr.statement
+        ndata = len(pr.weights) + len(shifts) + 2 * self.nregs * blen
+        nitems = len(pr.top) * (4 + 2 * self.nregs)
+        return (npath * (64 + 16 + 8 + 4 + 8 + 4) + 64 * ndigest + ncol * (4 * 16 + 8 + 4 + 4) +
+                16 * (nitems + ndata) + 4 * len(pr.top) + self.last_len * (16 + 128 + 16) + 8 + 64 + 11 * 16)
+
+    def _chunks(self, parsed):
+        """runs of consecutive proofs whose device buffers (_bytes) stay within CHUNK_BYTES; a proof above the bound
+        on its own is a chunk of its own"""
+        chunks, cur, used = [], [], 0
+        for b, pr in parsed:
+            size = self._bytes(pr)
+            if cur and used + size > CHUNK_BYTES:
+                chunks.append(cur)
+                cur, used = [], 0
+            cur.append((b, pr))
+            used += size
+        return chunks + ([cur] if cur else [])
+
+    def verify_batch(self, proofs, boundaries, proof_streams=None, reasons=False):
+        """The reference's verdict for each (proofs[b], boundaries[b], proof_streams[b]) (each proof's stream
+        deserializes it, so a SignatureProofStream's prefix enters its Fiat-Shamir): a list of bool, or with
+        `reasons` of (bool, reason) pairs, the reason None for an accepted proof, else the message the reference
+        prints for the first failing check (its three lines for the last codeword's degree), "leaf path" for an
+        opened leaf's path, "combination" for the combination and "malformed" for a stream outside the shape.  A
+        zero transition zerofier value at a checked index raises the reference's AssertionError("divide by zero")
+        with the proof's index as ``proof_index``, as verifying the proofs one at a time in order would."""
+        proofs, boundaries = list(proofs), list(boundaries)
+        B = len(proofs)
+        assert len(boundaries) == B, "sa_stark: %d proofs and %d boundaries" % (B, len(boundaries))
+        streams = [None] * B if proof_streams is None else list(proof_streams)
+        assert len(streams) == B, "sa_stark: %d proofs and %d proof streams" % (B, len(streams))
+        out = [None] * B
+        parsed = []
+        for b in range(B):
+            try:
+                pr = self._parse(proofs[b], boundaries[b], streams[b])
+            except Exception as exc:
+                exc.proof_index = b
+                raise
+            if pr is None:
+                out[b] = (False, MALFORMED)
+            else:
+                parsed.append((b, pr))
+        eng = sa_engine.get_engine()
+        for chunk in self._chunks(parsed):
+            raw, L = self._pack([pr for _, pr in chunk])
+            mflags, cflags, kflags, degrees, roots = eng.verify_chunk(eng.upload_bytes(raw), L)
+            m = c = q = 0
+            ktop = L["k"]
+            for j, (b, pr) in enumerate(chunk):
+                nm = (self.rounds - 1) * 3 * self.k + sum(len(reads) for _, reads in pr.opened)
+                nc = (self.rounds - 1) * self.k
+                try:
+                    out[b] = self._decide(pr, mflags[m:m + nm], cflags[c:c + nc], kflags[q:q + ktop], degrees[j],
+                                          roots[64 * j:64 * (j + 1)])
+                except AssertionError as exc:
+                    exc.proof_index = b
+                    raise
+                m, c, q = m + nm, c + nc, q + ktop
+        return out if reasons else [v for v, _ in out]
+
+    def verify(self, proof, boundary, proof_stream=None):
+        """verify_batch of one proof: its bool"""
+        return self.verify_batch([proof], [boundary], None if proof_stream is None else [proof_stream])[0]
+
+
 _originals = {}  # class -> its own `prove` attribute before enable (None: inherited)
+_verify_originals = {}  # class -> (its own `verify` attribute before enable_verify (None: inherited), the method)
 
 
 def enable(cls):
@@ -824,11 +1228,67 @@ def enable_plain(cls):
         cls.prove = prove_plain
 
 
+def _verify_on_plan(original, make_plan, proof, boundary, proof_stream, args):
+    """the plan's verdict, the reference's message printed where it prints one.  A Stark the plan refuses (more
+    than 16 registers, a shift at or above 2^32, a plain Stark of one cycle) and a malformed stream go to the
+    class's original verify, so its behaviour, exceptions included, is the reference's"""
+    try:
+        plan = make_plan()  # an AIR the program compiler refuses raises SaError, an AssertionError too
+    except AssertionError:
+        return original(*args)
+    try:
+        verdict, reason = plan.verify_batch([proof], [boundary], [proof_stream], reasons=True)[0]
+    except _Refused:
+        return original(*args)
+    if reason == MALFORMED:
+        return original(*args)
+    if reason is not None and reason not in ("leaf path", "combination"):
+        print(reason)
+    return verdict
+
+
+def enable_verify(cls):
+    """rebind cls.verify (FastStark's, or a subclass's) to a VerifierPlan built for the call (idempotent), so that
+    FastRPSSS.verify runs unmodified; a stream outside the shape is verified by the original method"""
+    if cls in _verify_originals:
+        return
+    original = cls.verify
+
+    def verify(self, proof, transition_constraints, boundary, transition_zerofier_root, proof_stream=None):
+        plan = lambda: VerifierPlan(self, transition_constraints, transition_zerofier_root)  # noqa: E731
+        return _verify_on_plan(original, plan, proof, boundary, proof_stream,
+                               (self, proof, transition_constraints, boundary, transition_zerofier_root,
+                                proof_stream))
+    _verify_originals[cls] = (cls.__dict__.get("verify"), original)
+    cls.verify = verify
+
+
+def enable_verify_plain(cls):
+    """rebind cls.verify (Stark's, or a subclass's) to a plain VerifierPlan built for the call (idempotent), so
+    that RPSSS.verify runs unmodified; a stream outside the shape is verified by the original method"""
+    if cls in _verify_originals:
+        return
+    original = cls.verify
+
+    def verify(self, proof, transition_constraints, boundary, proof_stream=None):
+        plan = lambda: VerifierPlan(self, transition_constraints)  # noqa: E731
+        return _verify_on_plan(original, plan, proof, boundary, proof_stream,
+                               (self, proof, transition_constraints, boundary, proof_stream))
+    _verify_originals[cls] = (cls.__dict__.get("verify"), original)
+    cls.verify = verify
+
+
 def disable():
-    """restore every class enable and enable_plain rebound"""
+    """restore every class enable, enable_plain, enable_verify and enable_verify_plain rebound"""
     for cls, orig in _originals.items():
         if orig is None:
             del cls.prove
         else:
             cls.prove = orig
     _originals.clear()
+    for cls, (orig, _) in _verify_originals.items():
+        if orig is None:
+            del cls.verify
+        else:
+            cls.verify = orig
+    _verify_originals.clear()
