@@ -468,6 +468,28 @@ int sa_fri_commit(void *layers, void *trees, const void *codeword, size_t n, int
                   const uint64_t offset[2], const uint64_t omega[2], sa_fri_challenge_fn challenge, void *user,
                   void *stream);
 
+/* ---- sa_fri_commit for `batch` codewords of one length n, one offset and one omega ----------
+ * codewords[b*n .. b*n+n) is codeword b.  Round 0 is one tree ladder over the B codewords, every
+ * later round one fused fold + tree ladder over all B rows, row b folding with its own alpha.
+ * After each round the host waits once for the round's B roots, then calls
+ * challenge(user, round, roots, alphas_out, want_alpha) once: roots holds B roots of 64 bytes
+ * back to back, and when want_alpha != 0 the callback writes alpha b as two limbs at
+ * alphas_out[2b], alphas_out[2b+1].  A non-zero return gives SA_ECALLBACK and nothing more is
+ * launched.  The launches of a round are those of one codeword, per group of 65535 codewords.
+ *   layers : rounds 1 .. rounds-1, round r as B back-to-back rows of n >> r elements, round after
+ *            round;  total B * (n - (n >> (rounds-1))) elements (unused, may be NULL, for rounds 1)
+ *   trees  : rounds 0 .. rounds-1, round r as B back-to-back trees of 2 (n >> r) nodes of 64 bytes
+ *            (sa_merkle_tree_batch's layout), round after round;  total B * (4n - (4n >> rounds))
+ *            nodes.  So sa_gather_batch_sets and sa_merkle_open_batch_sets with group = 1 open
+ *            each row of a round at its own indices.
+ * Before any launch: SA_ESIZE for n not a power of two, rounds < 1, rounds > log2(n) + 1, and a
+ * NULL buffer, offset, omega or callback; batch == 0 returns SA_OK without work.              */
+typedef int (*sa_fri_challenge_batch_fn)(void *user, int round, const uint8_t *roots, uint64_t *alphas_out,
+                                         int want_alpha);
+int sa_fri_commit_batch(void *layers, void *trees, const void *codewords, size_t n, size_t batch, int rounds,
+                        const uint64_t offset[2], const uint64_t omega[2], sa_fri_challenge_batch_fn challenge,
+                        void *user, void *stream);
+
 /* ---- seeded randomizer draws (code/algebra.py:118-120 field.sample(os.urandom(17))) -------------
  * For a 32-byte seed s, draw j (a uint64) is the element field.sample gives when os.urandom(17) returns
  * blake2b(s || j as 8 little-endian bytes).digest()[:17] (64-byte digest, no key): that digest's first 17 bytes

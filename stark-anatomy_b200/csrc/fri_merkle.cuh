@@ -1,10 +1,12 @@
 // fri_merkle.cuh -- per-thread pieces of the FRI round kernel: split-and-fold
 // (code/fri.py:85) and the chunked Merkle reduction (code/merkle.py:6-14).
-// __host__ __device__ so tests/emu can drive the same code phase by phase; the launch loop of a tree
-// and the fold scalars are shared with it too.
+// __host__ __device__ so tests/emu can drive the same code phase by phase; the launch loop of a tree,
+// the fold scalars and the round loop of the batched commit are shared with it too.
 #pragma once
 #include <algorithm>
 #include <cstdio>
+#include <cstring>
+#include <vector>
 
 #include "field.cuh"
 #include "hash.cuh"
@@ -38,7 +40,8 @@ SA_HD fe merkle_ld_stream(const fe *p) {
 struct MerkleArgs {
     uint64_t *tree;      // heap layout, 8 words per node; tree b of a batch at tree + b * tree_stride
     long long tree_stride;  // words from one tree of a batch to the next (16 per leaf), 0 without a batch
-    long long row_stride;   // mode 1: elements from one codeword row of a batch to the next
+    long long row_stride;   // elements from one row of a batch to the next: mode 1 `values`, mode 2 `next`
+                            // (mode 2 `prev` rows are twice as long)
     long long width;     // number of bottom nodes of this launch
     int chunk;           // bottom nodes per CTA (power of two, <= MK_THREADS << ipt_log)
     int ipt_log;         // log2 of the bottom nodes one thread reduces privately (0..3)
@@ -51,20 +54,32 @@ struct MerkleArgs {
     fe *next;            // mode 2: receives the folded codeword (width elements)
     const fe *xinv;      // mode 2: xinv[i] = omega^-i in Montgomery form, i < width
     fe s_m;              // mode 2: alpha * 2^-1 * offset^-1 in Montgomery form
+    const fe *s_rows;    // mode 2, optional: tree b of a batch folds with s_rows[b] instead of s_m (device memory)
     fe inv2_m;           // mode 2: 2^-1 in Montgomery form
     unsigned int *ticket;  // optional: CTA arrival counters, one per tree (zero between launches); the CTA of a
                          // tree that arrives last also reduces its gridDim.x (<= MK_THREADS) subtree roots,
                          // saving a launch
-    uint64_t *root_out;  // last launch of a single tree, optional: host-mapped landing pad, receives the root
-    unsigned long long root_seq;  // (8 words) and then this sequence number in word 8
+    uint64_t *root_out;  // last launch of a tree, optional: host-mapped landing pad, receives the root (8 words)
+    unsigned long long root_seq;  // and then this sequence number in word 8; tree b of a batch at root_out + 9 b
 };
 
-// the arguments of tree b of a batch: its nodes, its codeword row and its arrival counter
+// the arguments of tree b of a batch: its nodes, its codeword rows, its fold scalar, its arrival counter and its
+// landing pad (pointer arithmetic only: the host computes the views of a launch group)
 SA_HD MerkleArgs merkle_view(const MerkleArgs &a, long long b) {
     MerkleArgs v = a;
     v.tree += b * a.tree_stride;
     v.values += b * a.row_stride;
+    v.prev += 2 * b * a.row_stride;
+    v.next += b * a.row_stride;
+    if (v.s_rows) v.s_rows += b;
     if (v.ticket) v.ticket += b;
+    if (v.root_out) v.root_out += 9 * b;
+    return v;
+}
+// what the CTAs of tree b work with: its view, with its own fold scalar read once
+SA_HD MerkleArgs merkle_tree_args(const MerkleArgs &a, long long b) {
+    MerkleArgs v = merkle_view(a, b);
+    if (v.s_rows) v.s_m = v.s_rows[0];
     return v;
 }
 
@@ -170,6 +185,76 @@ inline void fri_fold_scalars(fe *s_m, fe *inv2_m, const fe &alpha, const fe &oin
     static const fe inv2 = fe_mont_inv(fe_to_mont(fe_from_u64(2)));
     *inv2_m = inv2;
     *s_m = fe_montmul(fe_montmul(fe_to_mont(alpha), inv2), oinv_m);
+}
+
+// ---- the batched FRI commit (sa_fri_commit_batch): B codewords of one length, offset and omega ----
+// Round r's B layers are back-to-back rows of n >> r elements (round 0's are the codewords), its B trees back-to-back
+// heaps of 2 (n >> r) nodes, round after round.  Round 0 is one tree ladder over the B codewords, every later round
+// one fused fold + tree ladder (mode 2) over the B rows of the previous round, each row folding with its own
+// challenge.  ops supplies what the device and the emulation do differently:
+//   ops.tree(a, r)                  the launches of round r's trees (merkle_batch_launches over the views of a)
+//   ops.roots(r, out)               waits once for round r's B roots, 64 bytes each, into out
+//   ops.challenge(r, roots, alphas, want)   the caller's callback: B alphas (two limbs each) when want
+//   ops.xinv(&tab, omega, len)      xinv[i] = omega^-i in Montgomery form, i < len / 2
+//   ops.scalars(&dev, r, host)      the B fold scalars of round r where the fold reads them
+// Returns SA_OK, SA_ECALLBACK when the callback returns non-zero (nothing more is launched), or ops' error.
+// sa_fri_commit_batch's refusals (SA_ESIZE); SA_OK for a batch of none whatever its buffers
+inline int fri_commit_batch_check(const void *layers, const void *trees, const void *codewords, size_t n, size_t batch,
+                                  int rounds, const void *offset, const void *omega, const void *challenge) {
+    if (!host_is_pow2(n) || rounds < 1 || rounds - 1 > host_log2(n)) return SA_ESIZE;
+    if (batch != 0 && (!trees || !codewords || (rounds > 1 && !layers) || !offset || !omega || !challenge))
+        return SA_ESIZE;
+    return SA_OK;
+}
+template <class Ops>
+int fri_commit_batch_rounds(Ops &&ops, fe *layers, uint64_t *trees, const fe *codewords, long long n, long long batch,
+                            int rounds, fe offset, fe omega) {
+    std::vector<uint8_t> roots((size_t)(64 * batch));
+    std::vector<uint64_t> alphas((size_t)(2 * batch));
+    std::vector<fe> s((size_t)batch);
+    fe oinv_m = fe_mont_inv(fe_to_mont(offset));  // squared along with offset (fri_fold_scalars)
+    const fe *cur = codewords;
+    long long len = n;
+    MerkleArgs a;
+    memset(&a, 0, sizeof(a));
+    a.tree = trees;
+    a.tree_stride = 16 * len;
+    a.row_stride = len;
+    a.width = len;
+    a.mode = 1;
+    a.values = cur;
+    for (int r = 0;; r++) {
+        SA_TRY(ops.tree(a, r));
+        SA_TRY(ops.roots(r, roots.data()));
+        const int want = r != rounds - 1;
+        if (ops.challenge(r, (const uint8_t *)roots.data(), alphas.data(), want) != 0) return SA_ECALLBACK;
+        if (!want) return SA_OK;
+        const fe *xinv = nullptr;
+        SA_TRY(ops.xinv(&xinv, omega, len));
+        fe inv2_m;
+        for (long long b = 0; b < batch; b++) fri_fold_scalars(&s[b], &inv2_m, fe_from_limbs(&alphas[2 * b]), oinv_m);
+        const fe *s_rows = nullptr;
+        SA_TRY(ops.scalars(&s_rows, r, s.data()));
+        // fold round r's rows into round r + 1's and build their trees
+        uint64_t *next_tree = a.tree + batch * 16 * len;
+        fe *next = layers;
+        layers += batch * (len / 2);
+        memset(&a, 0, sizeof(a));
+        a.tree = next_tree;
+        a.tree_stride = 8 * len;
+        a.row_stride = len / 2;
+        a.width = len / 2;
+        a.mode = 2;
+        a.prev = cur;
+        a.next = next;
+        a.xinv = xinv;
+        a.s_rows = s_rows;
+        a.inv2_m = inv2_m;
+        cur = next;
+        len /= 2;
+        omega = fe_montmul(fe_to_mont(omega), omega);  // omega^2 (Montgomery form times canonical = canonical)
+        oinv_m = fe_montmul(oinv_m, oinv_m);           // (offset^2)^-1
+    }
 }
 
 // digest of bottom node g of this launch: loads it (mode 0) or hashes the leaf (modes 1, 2) and

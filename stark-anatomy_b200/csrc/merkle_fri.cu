@@ -48,7 +48,7 @@ __device__ __forceinline__ void merkle_publish_root(const MerkleArgs &a, const u
 // single tree.
 __global__ void __launch_bounds__(MK_THREADS, 2) k_merkle_chunk(const __grid_constant__ MerkleArgs args) {
     __shared__ uint64_t sm[MK_THREADS * 8];
-    const MerkleArgs a = merkle_view(args, blockIdx.y);
+    const MerkleArgs a = merkle_tree_args(args, blockIdx.y);
     const long long blk = blockIdx.x;
     const unsigned nblocks = gridDim.x;
     const int tid = threadIdx.x;
@@ -225,7 +225,7 @@ static unsigned int *get_tickets(cudaStream_t st, int trees) {
     }
     return slot.ptr;  // nullptr: fall back to one more launch
 }
-// the launches of `batch` trees, merkle_view's layout; root_host: publish the root of a single tree there
+// the launches of `batch` trees, merkle_view's layout; root_host: tree b publishes its root at root_host + 9 b
 static int merkle_reduce(MerkleArgs a, size_t batch, cudaStream_t st, uint64_t *root_host = nullptr,
                          unsigned long long seq = 0) {
 #ifdef SA_TUNE
@@ -233,13 +233,14 @@ static int merkle_reduce(MerkleArgs a, size_t batch, cudaStream_t st, uint64_t *
 #else
     const char *shape_spec = nullptr;
 #endif
-    if (root_host && batch != 1) return SA_ESIZE;
+    a.root_out = root_host;  // (merkle_view offsets it per launch group)
+    a.root_seq = seq;
     return merkle_batch_launches(
         a, (long long)batch, [&](int trees) { return get_tickets(st, trees); }, shape_spec,
         [&](MerkleArgs &m, int trees, bool last) -> int {
-            m.root_out = last ? root_host : nullptr;
-            m.root_seq = seq;
-            k_merkle_chunk<<<dim3((unsigned)(m.width / m.chunk), (unsigned)trees), MK_THREADS, 0, st>>>(m);
+            MerkleArgs k = m;
+            if (!last) k.root_out = nullptr;  // only the launch that finishes the trees publishes
+            k_merkle_chunk<<<dim3((unsigned)(k.width / k.chunk), (unsigned)trees), MK_THREADS, 0, st>>>(k);
             SA_LAUNCH_CHECK();
             return SA_OK;
         });
@@ -480,6 +481,85 @@ int sa_fri_commit(void *layers, void *trees, const void *codeword, size_t n, int
         oinv_m = fe_montmul(oinv_m, oinv_m);  // (offset^2)^-1, stays in Montgomery form
     }
     return SA_OK;
+}
+
+// what sa_fri_commit_batch keeps between calls of a thread: pinned, mapped host memory holding the landing pads of
+// a round's roots (9 words per tree, merkle_publish_root) and then every round's fold scalars, which each round
+// copies to the device in stream order
+struct FriBatchHost {
+    uint64_t *pinned = nullptr;
+    size_t bytes = 0;
+    unsigned long long seq = 0;  // the sequence number of the last round published
+};
+
+int sa_fri_commit_batch(void *layers, void *trees, const void *codewords, size_t n, size_t batch, int rounds,
+                        const uint64_t offset[2], const uint64_t omega[2], sa_fri_challenge_batch_fn challenge,
+                        void *user, void *stream) {
+    SA_TRY(fri_commit_batch_check(layers, trees, codewords, n, batch, rounds, offset, omega, (const void *)challenge));
+    if (batch == 0) return SA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    static thread_local FriBatchHost host;
+    const size_t pad_words = 9 * batch, need = 8 * pad_words + sizeof(fe) * batch * (size_t)(rounds - 1);
+    if (host.bytes < need) {
+        if (host.pinned) {
+            SA_CUDA(cudaFreeHost(host.pinned));
+            host = FriBatchHost{nullptr, 0, host.seq};
+        }
+        SA_CUDA(cudaHostAlloc((void **)&host.pinned, need, cudaHostAllocMapped | cudaHostAllocPortable));
+        memset(host.pinned, 0, need);  // no sequence number is 0
+        host.bytes = need;
+    }
+    uint64_t *pad_dev = nullptr;
+    SA_CUDA(cudaHostGetDevicePointer((void **)&pad_dev, host.pinned, 0));  // per current device
+    fe *s_host = (fe *)(host.pinned + pad_words);
+    fe *s_dev = nullptr;  // every round's scalars, freed in stream order whatever the outcome
+    if (rounds > 1) {
+        keep_pool_memory();
+        SA_CUDA(cudaMallocAsync((void **)&s_dev, sizeof(fe) * batch * (size_t)(rounds - 1), st));
+    }
+    struct Free {
+        fe *p;
+        cudaStream_t st;
+        ~Free() {
+            if (p) cudaFreeAsync(p, st);
+        }
+    } free_s{s_dev, st};
+    const long long B = (long long)batch;
+    XinvPtr xinv;  // keeps the current round's table alive
+    struct Ops {
+        long long B;
+        cudaStream_t st;
+        uint64_t *pad_host, *pad_dev;
+        unsigned long long &seq;
+        fe *s_host, *s_dev;
+        XinvPtr &tab;
+        sa_fri_challenge_batch_fn fn;
+        void *user;
+        int tree(const MerkleArgs &a, int) { return merkle_reduce(a, (size_t)B, st, pad_dev, ++seq); }
+        int roots(int, uint8_t *out) {
+            for (long long b = 0; b < B; b++) {  // the one wait of the round: every tree's sequence word
+                SA_TRY(wait_for_root(pad_host + 9 * b, seq, st));
+                memcpy(out + 64 * b, pad_host + 9 * b, 64);
+            }
+            return SA_OK;
+        }
+        int challenge(int r, const uint8_t *roots, uint64_t *alphas, int want) { return fn(user, r, roots, alphas, want); }
+        int xinv(const fe **out, const fe &omega, long long len) {
+            SA_TRY(get_xinv(&tab, omega, (size_t)len, st));
+            *out = tab->tab;
+            return SA_OK;
+        }
+        int scalars(const fe **dev, int r, const fe *host) {
+            fe *h = s_host + (size_t)r * B, *d = s_dev + (size_t)r * B;
+            memcpy(h, host, sizeof(fe) * B);
+            SA_CUDA(cudaMemcpyAsync(d, h, sizeof(fe) * B, cudaMemcpyHostToDevice, st));
+            *dev = d;
+            return SA_OK;
+        }
+    };
+    return fri_commit_batch_rounds(Ops{B, st, host.pinned, pad_dev, host.seq, s_host, s_dev, xinv, challenge, user},
+                                   (fe *)layers, (uint64_t *)trees, (const fe *)codewords, (long long)n, B, rounds,
+                                   fe_from_limbs(offset), fe_from_limbs(omega));
 }
 
 }  // extern "C"

@@ -39,6 +39,7 @@ from ntt import intt
 import sa_engine
 import sa_devlist
 from sa_devlist import DeviceCodeword
+import sa_marshal
 
 
 class Merkle(_HostMerkle):
@@ -250,6 +251,127 @@ class Fri:
             self.query(codewords[i], codewords[i + 1], indices, proof_stream)
 
         return top_level_indices
+
+    # -------------------------------------------------------------- batches --
+    def _commit_batch(self, codewords, proof_streams, field):
+        """commit_batch, and the (B, N >> r, 2) device layers and (B, 2 (N >> r), 64) trees of every round"""
+        eng = sa_engine.get_engine()
+        p = self.field.p
+        B = len(proof_streams)
+        if hasattr(codewords, "shape"):  # one (B, N, 2) device tensor
+            vecs = codewords
+            assert len(vecs.shape) == 3 and vecs.shape[0] == B, "fri: %d rows and %d proof streams" % (vecs.shape[0], B)
+            N = vecs.shape[1]
+            if B == 0:
+                return [], [], []
+            first = [DeviceCodeword(vecs[b], None, field or self.field, N) for b in range(B)]
+        else:
+            first = list(codewords)
+            assert len(first) == B, "fri: %d codewords and %d proof streams" % (len(first), B)
+            N = len(first[0]) if first else 0
+            assert all(len(cw) == N for cw in first), "fri: the codewords of a batch differ in length"
+            if B == 0:
+                return [], [], []
+            if any(isinstance(cw, DeviceCodeword) for cw in first):
+                vecs = eng.concat([sa_devlist.to_device(cw) for cw in first]).reshape(B, N, 2)
+            else:  # one upload
+                vecs = eng.upload(bytearray().join(sa_devlist.pack(cw) for cw in first)).reshape(B, N, 2)
+        self._resident = {}
+        rounds = self.num_rounds()
+        assert(pow(self.omega.value, N - 1, p) == pow(self.omega.value, -1, p)), "error in commit: omega does not have the right order!"
+
+        def on_roots(r, roots, want_alpha):
+            # stream by stream: its root (fri.py:71-72), then its challenge (fri.py:79)
+            alphas = []
+            for ps, root in zip(proof_streams, roots):
+                ps.push(root)
+                if want_alpha:
+                    alphas.append(self.field.sample(ps.prover_fiat_shamir()).value)
+            return alphas
+
+        layers, trees = eng.fri_commit_batch(vecs, rounds, self.offset.value, self.omega.value, on_roots)
+        # every proof's last codeword as a real list (it is pickled into the transcript), from one download; a lone
+        # round's last codeword is the caller's own
+        if rounds > 1 or hasattr(codewords, "shape"):
+            raw = eng.download(layers[-1].reshape(-1, 2)).reshape(B, -1, 2)
+            last = [sa_marshal.unpack(raw[b], self.field if rounds > 1 else sa_devlist.field_of(first[b]), FieldElement)
+                    for b in range(B)]
+        else:
+            last = [cw.tolist() if isinstance(cw, DeviceCodeword) else cw for cw in first]
+        out = []
+        for b, ps in enumerate(proof_streams):
+            if isinstance(first[b], DeviceCodeword):
+                first[b].attach_tree(trees[0][b])
+            cws = [first[b]] + [DeviceCodeword(layers[r][b], trees[r][b], self.field, N >> r) for r in range(1, rounds)]
+            cws[-1] = last[b]
+            ps.push(cws[-1])
+            out.append(cws)
+        return out, layers, trees
+
+    def commit_batch(self, codewords, proof_streams, field=None):
+        """``commit(codewords[b], proof_streams[b])`` for every b as one batched commit (sa_fri_commit_batch): every
+        stream receives the objects ``commit`` pushes, the streams visited in order each round, and one host wait per
+        round serves the whole batch.  `codewords` is a list of lists or DeviceCodewords of one length, or one
+        (B, N, 2) device tensor whose rows hold elements of `field` (default: this Fri's).  Returns each proof's
+        codewords as ``commit`` returns them."""
+        return self._commit_batch(codewords, proof_streams, field)[0]
+
+    def prove_batch(self, codewords, proof_streams, field=None):
+        """``prove(codewords[b], proof_streams[b])`` for every b: each stream receives exactly the objects ``prove``
+        pushes (so ``pickle.dumps(ps.objects)`` is the same), with the commit of ``commit_batch`` and, per layer, one
+        gather and one path read for the whole batch.  Inputs as ``commit_batch`` takes them.  Returns each proof's
+        top-level indices."""
+        eng = sa_engine.get_engine()
+        B = len(proof_streams)
+        if hasattr(codewords, "shape"):
+            assert(codewords.shape[1] == self.domain_length), "initial codeword length does not match length of initial codeword"
+        else:
+            for cw in codewords:
+                assert(self.domain_length == len(cw)), "initial codeword length does not match length of initial codeword"
+        if B == 0:
+            return []
+        cws, layers, trees = self._commit_batch(codewords, proof_streams, field)
+        rounds = len(cws[0])
+        N, k = self.domain_length, self.num_colinearity_tests
+        tops = [self.sample_indices(ps.prover_fiat_shamir(), N // 2, len(cws[b][-1]), k)
+                for b, ps in enumerate(proof_streams)]
+        if rounds == 1:
+            return tops
+        # the c indices of every query round (fri.py:116), then each layer's openings: c of the round before it, a and
+        # b of its own round
+        cs = [[[i % ((N >> r) // 2) for i in top] for top in tops] for r in range(rounds - 1)]
+        sets = []
+        for r in range(rounds):
+            sets.append([(cs[r - 1][b] if r else []) + (cs[r][b] + [i + (N >> r) // 2 for i in cs[r][b]]
+                                                        if r < rounds - 1 else []) for b in range(B)])
+        values, paths = [], []
+        for r in range(rounds):
+            paths.append(eng.merkle_open_batch(trees[r], sets[r], group=1))
+            if r == rounds - 1:  # the pushed last codewords' own elements
+                values.append([[cws[b][r][i] for i in sets[r][b]] for b in range(B)])
+                continue
+            raw = eng.gather_batch(layers[r], sets[r], group=1)
+            row = []
+            for b in range(B):
+                layer = cws[b][r]
+                if isinstance(layer, DeviceCodeword):
+                    row.append(layer.adopt(sets[r][b], sa_marshal.unpack(raw[b], sa_devlist.field_of(layer),
+                                                                         FieldElement)))
+                else:
+                    row.append([layer[i] for i in sets[r][b]])
+            values.append(row)
+        for r in range(rounds - 1):
+            cur_at = k if r else 0  # layer r's a and b openings follow its c openings of round r - 1
+            for b, ps in enumerate(proof_streams):
+                cur, cur_paths = values[r][b][cur_at:], paths[r][b][cur_at:]
+                nxt, nxt_paths = values[r + 1][b][:k], paths[r + 1][b][:k]
+                for s in range(k):
+                    ps.push((cur[s], cur[k + s], nxt[s]))
+                for s in range(k):
+                    ps.push(cur_paths[s])
+                    ps.push(cur_paths[k + s])
+                    ps.push(nxt_paths[s])
+        return tops
 
     # --------------------------------------------------------------- verify --
     def verify(self, proof_stream, polynomial_values):

@@ -113,6 +113,14 @@ class DeviceCodeword:
         for i, el in zip(missing, sa_marshal.unpack(raw, self._field, FieldElement)):
             self._cache[i] = el
 
+    def adopt(self, indices, elements):
+        """the element objects at `indices` given their values read elsewhere (`elements`, one per index, e.g. from
+        one gather over many device lists): those handed out earlier where there are, else the given ones, which are
+        handed out from then on"""
+        if self._full is not None:
+            return [self._full[i] for i in indices]
+        return [self._cache.setdefault(i, el) for i, el in zip(indices, elements)]
+
     def tolist(self):
         if self._full is None:
             full = from_device(self._vec, self._field)

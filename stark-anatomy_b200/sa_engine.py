@@ -108,6 +108,7 @@ SYMBOLS = [
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_commit", _ci, [_vp, _vp, _vp, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
+    ("sa_fri_commit_batch", _ci, [_vp, _vp, _vp, _sz, _sz, _ci, _u64p, _u64p, _vp, _vp, _vp]),
     ("sa_cache_limit", _sz, [_sz]),
     ("sa_cache_bytes", _sz, []),
     ("sa_release_workspaces", _ci, []),
@@ -1046,6 +1047,57 @@ class CudaEngine:
             if r + 1 < rounds:
                 out_layers.append(layers[lo:lo + ln // 2])
                 lo += ln // 2
+                ln //= 2
+        return out_layers, out_trees
+
+    def fri_commit_batch(self, vecs, rounds, offset, omega, on_roots):
+        """sa_fri_commit_batch: fri_commit for the B rows of a (B, n, 2) device tensor in one launch ladder.
+
+        on_roots(round, roots, want_alpha) is called once per round with the B 64-byte roots of the round (a list of
+        bytes, from one host wait); it returns the B challenges (ints) when want_alpha.  Returns (layers, trees):
+        layers[r] the (B, n >> r, 2) rows of round r (layers[0] is `vecs`), trees[r] their (B, 2 (n >> r), 64) trees,
+        views of one layer buffer and one tree buffer laid out as the library lays them."""
+        torch = self.torch
+        if vecs.dim() != 3 or vecs.shape[-1] != 2 or vecs.dtype != torch.int64:
+            raise SaError(SA_ERRORS[-6])
+        vecs = vecs.contiguous()
+        batch, n = vecs.shape[0], vecs.shape[1]
+        if n < 1 or n & (n - 1) or not 1 <= rounds <= n.bit_length():
+            raise SaError(SA_ERRORS[-6])
+        layers = self.empty(max(batch * (n - (n >> (rounds - 1))), 1))
+        trees = torch.empty((max(batch * (4 * n - ((4 * n) >> rounds)), 1), 64), dtype=torch.uint8, device=self.device)
+        errors = []
+
+        def challenge(_user, r, roots_ptr, alphas_out, want):
+            try:
+                self._count("d2h", 64 * batch)  # the round's roots, from the mapped landing pads
+                raw = ctypes.string_at(roots_ptr, 64 * batch)
+                alphas = on_roots(r, [raw[64 * b:64 * (b + 1)] for b in range(batch)], bool(want))
+                if want:
+                    alphas = list(alphas)
+                    if len(alphas) != batch:
+                        raise ValueError("fri_commit_batch: %d challenges for %d codewords" % (len(alphas), batch))
+                    for b, alpha in enumerate(alphas):
+                        alphas_out[2 * b] = alpha & 0xFFFFFFFFFFFFFFFF
+                        alphas_out[2 * b + 1] = alpha >> 64
+                return 0
+            except BaseException as exc:  # re-raised below, outside the C frame
+                errors.append(exc)
+                return 1
+        cb = FRI_CHALLENGE_FN(challenge)
+        rc = self.lib.sa_fri_commit_batch(layers.data_ptr(), trees.data_ptr(), vecs.data_ptr(), n, batch, rounds,
+                                          _limbs(offset), _limbs(omega), cb, None, self._stream())
+        if errors:
+            raise errors[0]
+        self._check(rc)
+        out_layers, out_trees = [vecs], []
+        lo, to, ln = 0, 0, n
+        for r in range(rounds):
+            out_trees.append(trees[to:to + batch * 2 * ln].view(batch, 2 * ln, 64))
+            to += batch * 2 * ln
+            if r + 1 < rounds:
+                out_layers.append(layers[lo:lo + batch * (ln // 2)].view(batch, ln // 2, 2))
+                lo += batch * (ln // 2)
                 ln //= 2
         return out_layers, out_trees
 

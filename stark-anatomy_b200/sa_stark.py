@@ -310,12 +310,14 @@ class _Stages:
         number = 1 + 2 * len(self.constraints) + 2 * self.nregs
         return [w.value for w in self.stark.sample_weights(number, proof_stream.prover_fiat_shamir())]
 
-    def _combine_prove_open(self, eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_streams):
+    def _combine_prove_open(self, eng, rvec, rows, bquot, bounds_b, weights, committed, trees, proof_streams,
+                            fri_batch=False):
         """for each proof b the combination of its randomizer, each transition quotient row (rows[b]: (the row
         truncated to its bound + 1, the bound)) and each boundary quotient at shift 0 and at max_degree - bound, all
-        B codewords from one call; FRI on each proof's codeword, proof by proof; then one gather and one path read
-        of every proof's committed codewords at that proof's own indices.  An empty row (a zero quotient) adds
-        nothing and is left out.  Returns each proof's quadrupled indices."""
+        B codewords from one call; FRI on each proof's codeword, proof by proof, or with fri_batch on all B rows of
+        the combination at once (Fri.prove_batch); then one gather and one path read of every proof's committed
+        codewords at that proof's own indices.  An empty row (a zero quotient) adds nothing and is left out.
+        Returns each proof's quadrupled indices."""
         stark, field, nregs, log_n, B = self.stark, self.stark.field, self.nregs, self.log_n, len(proof_streams)
         n = 1 << log_n
         terms = []
@@ -336,9 +338,13 @@ class _Stages:
         else:
             combined = eng.coset_combine_evaluate_batch(terms, B, *args)
 
+        if fri_batch:
+            tops = self.fri.prove_batch(combined, proof_streams, field)
+        else:
+            tops = [self.fri.prove(sa_devlist.DeviceCodeword(combined[b], None, field, n), ps)
+                    for b, ps in enumerate(proof_streams)]
         quadrupled = []
-        for b, ps in enumerate(proof_streams):
-            indices = self.fri.prove(sa_devlist.DeviceCodeword(combined[b], None, field, n), ps)
+        for indices in tops:
             duplicated = list(indices) + [(i + stark.expansion_factor) % n for i in indices]
             quadrupled.append(sorted(duplicated + [(i + n // 2) % n for i in duplicated]))
         # each proof's distinct indices, padded with its last one to a common length
@@ -361,13 +367,14 @@ class _Stages:
                     ps.push(paths[r][q])
         return quadrupled
 
-    def _prove_batch(self, traces, boundaries, proof_streams, transition, seeds=None, columns=None):
+    def _prove_batch(self, traces, boundaries, proof_streams, transition, seeds=None, columns=None, fri_batch=False):
         """the schedule both provers share: (the proof streams, each proof's quadrupled indices).  transition(eng,
         polys, failed, B) runs the plan's transition quotients and their checks for every proof not yet in `failed`
         and returns (rows_of, degree_check): rows_of(b) gives proof b's combination rows, degree_check(eng, live,
         failed) checks the proofs below `live`.  With `seeds` (one 32-byte seed per proof) every draw comes from the
         device expansion of its proof's seed and nothing calls os.urandom.  With `columns` (the (B nregs, T, 2)
-        device column buffer with every proof's trace in its first ncycles rows) `traces` is None."""
+        device column buffer with every proof's trace in its first ncycles rows) `traces` is None.  fri_batch runs FRI
+        on the whole batch at once (_combine_prove_open)."""
         B = len(traces) if columns is None else len(boundaries)
         seeds = _seeds(seeds, B)
         eng = sa_engine.get_engine()
@@ -387,7 +394,7 @@ class _Stages:
             b, exc = self._refused(eng, boundaries)
             self._prove_batch(None if columns is not None else traces[:b], boundaries[:b], proof_streams[:b],
                               transition, None if seeds is None else seeds[:b],
-                              None if columns is None else columns[:b * self.nregs])
+                              None if columns is None else columns[:b * self.nregs], fri_batch)
             exc.proof_index = b
             raise exc
         committed, bquot, bounds_b = stage
@@ -412,7 +419,7 @@ class _Stages:
             raise failed[b]
 
         quadrupled = self._combine_prove_open(eng, rvec, [rows_of(b) for b in range(B)], bquot, bounds_b, weights,
-                                              committed, trees, proof_streams)
+                                              committed, trees, proof_streams, fri_batch)
         return proof_streams, quadrupled
 
 
@@ -510,17 +517,21 @@ class StarkPlan(_Stages):
         return self.prove_batch([trace], [boundary], transition_zerofier_codeword,
                                 None if proof_stream is None else [proof_stream], None if seed is None else [seed])[0]
 
-    def prove_batch(self, traces, boundaries, transition_zerofier_codeword, proof_streams=None, seeds=None):
+    def prove_batch(self, traces, boundaries, transition_zerofier_codeword, proof_streams=None, seeds=None,
+                    fri_batch=False):
         """FastStark.prove for each (traces[b], boundaries[b], proof_streams[b]) with this plan's constraints and
         zerofier, the pre-FRI stages of all proofs in one schedule: the list of proof bytes, proof b's the bytes
         proving it alone gives from the same draws (DESIGN section 3.11 gives the draw order).  The exception is the
         one proving the proofs one at a time in order raises first, with the failing proof's index as
         ``proof_index``.  With `seeds`, one 32-byte seed per proof, proof b's draws are the device expansion of
         seeds[b] (DESIGN section 3.13): its bytes are those proving it alone with os.urandom = seeded_urandom(seeds[b])
-        gives, whatever the batch."""
-        return self._prove(list(traces), list(boundaries), transition_zerofier_codeword, proof_streams, seeds)
+        gives, whatever the batch.  With fri_batch, FRI runs on all proofs at once (Fri.prove_batch: one host wait per
+        round for the whole batch) and the proofs are the same bytes."""
+        return self._prove(list(traces), list(boundaries), transition_zerofier_codeword, proof_streams, seeds,
+                           fri_batch=fri_batch)
 
-    def _prove(self, traces, boundaries, transition_zerofier_codeword, proof_streams, seeds, columns=None):
+    def _prove(self, traces, boundaries, transition_zerofier_codeword, proof_streams, seeds, columns=None,
+               fri_batch=False):
         """prove_batch, or with `columns` (traces None) the proofs of the traces already in that column buffer"""
         T, nregs = self.trace_length, self.nregs
         where = self._where()
@@ -570,7 +581,8 @@ class StarkPlan(_Stages):
                 return [(quots[where[k.index][0]][b, where[k.index][1], :k.bound + 1], k.bound) for k in self.cons]
             return rows_of, degree_check
 
-        streams, quadrupled = self._prove_batch(traces, boundaries, proof_streams, transition, seeds, columns)
+        streams, quadrupled = self._prove_batch(traces, boundaries, proof_streams, transition, seeds, columns,
+                                                fri_batch)
 
         # ... and the zerofier's openings (:171-175), proof by proof: the codeword is the caller's
         zc = transition_zerofier_codeword
@@ -661,15 +673,15 @@ class PlainStarkPlan(_Stages):
         return self.prove_batch([trace], [boundary], None if proof_stream is None else [proof_stream],
                                 None if seed is None else [seed])[0]
 
-    def prove_batch(self, traces, boundaries, proof_streams=None, seeds=None):
+    def prove_batch(self, traces, boundaries, proof_streams=None, seeds=None, fri_batch=False):
         """Stark.prove for each (traces[b], boundaries[b], proof_streams[b]) with this plan's constraints, the
         pre-FRI stages of all proofs in one schedule: the list of proof bytes, proof b's the bytes proving it alone
         gives from the same draws (DESIGN section 3.11).  The exception is the one proving the proofs one at a time
         in order raises first, with the failing proof's index as ``proof_index``.  `seeds` as
-        StarkPlan.prove_batch's."""
-        return self._prove(list(traces), list(boundaries), proof_streams, seeds)
+        StarkPlan.prove_batch's, and fri_batch as there."""
+        return self._prove(list(traces), list(boundaries), proof_streams, seeds, fri_batch=fri_batch)
 
-    def _prove(self, traces, boundaries, proof_streams, seeds, columns=None):
+    def _prove(self, traces, boundaries, proof_streams, seeds, columns=None, fri_batch=False):
         """prove_batch, or with `columns` (traces None) the proofs of the traces already in that column buffer"""
         T, nregs = self.trace_length, self.nregs
 
@@ -718,7 +730,7 @@ class PlainStarkPlan(_Stages):
                 return rows
             return rows_of, degree_check
 
-        streams, _ = self._prove_batch(traces, boundaries, proof_streams, transition, seeds, columns)
+        streams, _ = self._prove_batch(traces, boundaries, proof_streams, transition, seeds, columns, fri_batch)
         return [ps.serialize() for ps in streams]
 
 
@@ -727,14 +739,15 @@ def prove_plain(stark, trace, transition_constraints, boundary, proof_stream=Non
     return PlainStarkPlan(stark, transition_constraints).prove(trace, boundary, proof_stream)
 
 
-def sign_batch(signer, sk, documents, seeds=None):
+def sign_batch(signer, sk, documents, seeds=None, fri_batch=False):
     """For an RPSSS or FastRPSSS instance `signer`, [signer.sign(sk, d) for d in documents]: each signature is the
     one signer.sign gives from the same draws, taken in prove_batch's order (signing draws nothing outside its
     prove).  The hash, the trace, the boundary and the transition constraints are computed once, one plan proves
     every document (PlainStarkPlan for a Stark, StarkPlan with the signer's zerofier for a FastStark), and each
     document's stream is the signer module's own SignatureProofStream.  Nothing is kept between calls.  With
     `seeds`, one secret 32-byte seed per document, signature d is signer.sign(sk, documents[d]) with os.urandom =
-    seeded_urandom(seeds[d]); a seed must never sign two different documents (DESIGN section 3.13)."""
+    seeded_urandom(seeds[d]); a seed must never sign two different documents (DESIGN section 3.13).  fri_batch as
+    StarkPlan.prove_batch's."""
     import sys
     documents = list(documents)
     seeds = _seeds(seeds, len(documents))
@@ -750,9 +763,9 @@ def sign_batch(signer, sk, documents, seeds=None):
     if hasattr(signer, "transition_zerofier"):
         plan = StarkPlan(stark, transition, signer.transition_zerofier)
         return plan.prove_batch([trace] * len(documents), [boundary] * len(documents),
-                                signer.transition_zerofier_codeword, streams, seeds)
+                                signer.transition_zerofier_codeword, streams, seeds, fri_batch)
     plan = PlainStarkPlan(stark, transition)
-    return plan.prove_batch([trace] * len(documents), [boundary] * len(documents), streams, seeds)
+    return plan.prove_batch([trace] * len(documents), [boundary] * len(documents), streams, seeds, fri_batch)
 
 
 class SignerPlan:
@@ -781,14 +794,14 @@ class SignerPlan:
         self.stream = sys.modules[type(signer).__module__].SignatureProofStream
         self._verifier = None
 
-    def sign(self, sks, documents, seeds=None):
+    def sign(self, sks, documents, seeds=None, fri_batch=False):
         """[signer.sign(sks[d], documents[d]) for each d]: one sa_rescue launch writes every key's trace into rows
         0 .. N of the prover's column buffer, the public keys are read from row N of register 0 with one gather, and
         the batch is proven as prove_batch proves it, each document with its own SignatureProofStream.  No trace
         element crosses to the device.  Unseeded, the draws are taken in prove_batch's order; with `seeds`, one
         secret 32-byte seed per signature, signature d is signer.sign(sks[d], documents[d]) with os.urandom =
         seeded_urandom(seeds[d]), whatever the batch.  Unequal lengths, bad seeds and keys that are not elements of p
-        raise an AssertionError before any device work."""
+        raise an AssertionError before any device work.  fri_batch as StarkPlan.prove_batch's."""
         sks, documents = list(sks), list(documents)
         assert len(sks) == len(documents), "sa_stark: %d keys and %d documents" % (len(sks), len(documents))
         seeds = _seeds(seeds, len(documents))
@@ -805,8 +818,8 @@ class SignerPlan:
         boundaries = [rp.boundary_constraints(element(_value(lo, hi), rp.field)) for lo, hi in pks.reshape(B, 2)]
         streams = [self.stream(d) for d in documents]
         if self.zerofier_codeword is not None:
-            return plan._prove(None, boundaries, self.zerofier_codeword, streams, seeds, columns)
-        return plan._prove(None, boundaries, streams, seeds, columns)
+            return plan._prove(None, boundaries, self.zerofier_codeword, streams, seeds, columns, fri_batch)
+        return plan._prove(None, boundaries, streams, seeds, columns, fri_batch)
 
 
     def verify(self, pks, documents, signatures, reasons=False):
