@@ -391,14 +391,25 @@ SA_HD void ntt_tile_full_stage(int t, fe *sm, const TileArgs &a, long long b, in
 #else
     (void)bar;
 #endif
-    // multiply output k by w_{M*R}^(k*m) = w_L^((k*m) << wlog), then park it in row row0 + k*M
+    // multiply output k by w_{M*R}^(k*m) = w_L^((k*m) << wlog), then park it in row row0 + k*M.  The stage
+    // before the last one (M = 2^LASTLOG) parks its outputs as they are and the last stage multiplies them as it
+    // loads them (ntt_tile_last_stage).  Here the factors of one (m = 0) belong to whole units, a quarter of the
+    // threads at M = 4; there they are the unrolled row d = 0 of every unit, so every thread and every warp skips
+    // the same share (a skip confined to some warps leaves the SM sub-partitions of the others just as busy)
     tile_st(sm + row0 * C + c, x[0]);
+    if (ml == P::LASTLOG) {
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-    for (int k = 1; k < R; k++) {
-        const fe w = tile_ld(tw + tile_tw_slot((k * m) << wlog));
-        tile_st(sm + (row0 + k * M) * C + c, tile_mul(x[k], w));
+        for (int k = 1; k < R; k++) tile_st(sm + (row0 + k * M) * C + c, x[k]);
+    } else {
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+        for (int k = 1; k < R; k++) {
+            const fe w = tile_ld(tw + tile_tw_slot((k * m) << wlog));
+            tile_st(sm + (row0 + k * M) * C + c, tile_mul(x[k], w));
+        }
     }
 }
 
@@ -432,7 +443,7 @@ SA_HD void ntt_tile_last_stage(int t, fe *sm, const TileArgs &a, long long b, in
     for (int s = 0; s < U; s++) {
         const int row0 = (q * U + s) * R;
         fe x[R];
-        if (FIRST) {
+        if constexpr (FIRST) {
             const fe *src = a.in + tile_batch_offset(b, a.inner, a.in_sb, a.in_sb2) + (long long)col * a.in_sc;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
@@ -443,6 +454,20 @@ SA_HD void ntt_tile_last_stage(int t, fe *sm, const TileArgs &a, long long b, in
 #pragma unroll
 #endif
             for (int d = 0; d < R; d++) x[d] = tile_ld(sm + (row0 + d) * C + c);
+            // the inter-stage twiddles of the stage before, which parked its outputs unmultiplied: row row0 + d
+            // is its output k = (row0 / R) mod E of unit m = d (that stage has M = R), so the factor is
+            // w_L^((k*d) << wlog) and row d = 0 has none
+            const fe *tw = a.tw;
+#if defined(__CUDA_ARCH__)
+            extern __shared__ uint4 sa_smem_u4[];
+            tw = reinterpret_cast<const fe *>(sa_smem_u4) + P::TILE_BYTES / sizeof(fe);
+#endif
+            constexpr int WLOG = LOGL - P::LASTLOG - P::EL;
+            const int k = (row0 >> P::LASTLOG) & (P::E - 1);
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+            for (int d = 1; d < R; d++) x[d] = tile_mul(x[d], tile_ld(tw + tile_tw_slot((k * d) << WLOG)));
         }
         dft_regs<R>(x, a.cst, CSTEP);
 #if defined(__CUDA_ARCH__)
