@@ -578,6 +578,30 @@ size_t sa_air_program_bytes(size_t nterms, size_t nregs);
 int sa_air_program(void *prog, const uint64_t *coeffs, const uint32_t *exps, const size_t *term_start, size_t ncons,
                    size_t nregs, void *stream);
 
+/* ---- proof transcripts from their pickled bytes (csrc/transcript.cuh, DESIGN section 3.17) ----------------------
+ * A verifier plan's shape is SA_TRANSCRIPT_SHAPE words: nregs, FRI rounds, k, the last codeword's length, log2 of
+ * the FRI domain, the opened codewords, the weights, the pickle protocol, the expansion factor and the memo capacity
+ * (see transcript.cuh for the shapes taken).  sa_transcript_bytes: one proof's device workspace in bytes, 0 for a
+ * shape refused.                                                                                                 */
+#define SA_TRANSCRIPT_SHAPE 10
+#define SA_TRANSCRIPT_SECTIONS 15
+#define SA_TRANSCRIPT_PREFIX 144 /* per proof: the prefix length (uint64), then at 16 up to 128 prefix bytes */
+#define SA_TRANSCRIPT_OUT 80     /* per proof: the accepted flag (uint32), then at 16 the last FRI root */
+size_t sa_transcript_bytes(const uint64_t shape[SA_TRANSCRIPT_SHAPE]);
+/* sa_transcript_sections: for nproofs proofs (proof b is proof_at[2b + 1] bytes at proofs + proof_at[2b]; device
+ * memory), parse each as the canonical pickle of a stream of the shape, hash its Fiat-Shamir messages with the
+ * prefix of prefixes + SA_TRANSCRIPT_PREFIX b, draw its weights, alphas and indices, and write the chunk sections
+ * VerifierPlan._pack writes at the byte offsets section_at of `sections` (zeroed by the caller): proof_data holds
+ * the weights, then nstat elements of `statement` per proof, and zroot (64 bytes, NULL without a zerofier codeword)
+ * is the root of the last opened codeword.  out gets SA_TRANSCRIPT_OUT bytes per proof.  A refused proof has flag
+ * 0 and zero values in its sections.  workspace: nproofs * sa_transcript_bytes(shape) bytes.  Six launches, no
+ * synchronisation.  SA_ESIZE before any launch for a refused shape, NULL buffers, nproofs or its products with the
+ * shape's sizes at or above 2^59, or a prefix longer than 128 bytes is read as a refusal of that proof.         */
+int sa_transcript_sections(void *sections, const uint64_t section_at[SA_TRANSCRIPT_SECTIONS], void *out,
+                           void *workspace, const void *proofs, const uint64_t *proof_at, const void *prefixes,
+                           const void *statement, size_t nstat, const void *zroot, size_t nproofs,
+                           const uint64_t shape[SA_TRANSCRIPT_SHAPE], void *stream);
+
 /* ---- self checks (used by tests / smoke) ------------------------------------------------
  * Runs the device carry-chain field arithmetic against the portable C++ version on
  * `count` pseudo-random pairs (plus edge cases) on the device; returns the number of

@@ -104,6 +104,8 @@ SYMBOLS = [
                                     _vp]),
     ("sa_poly_degree_batch", _ci, [_vp, _vp, _sz, _sz, _vp]),
     ("sa_air_program_bytes", _sz, [_sz, _sz]),
+    ("sa_transcript_bytes", _sz, [_u64p]),
+    ("sa_transcript_sections", _ci, [_vp, _u64p, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _sz, _u64p, _vp]),
     ("sa_air_program", _ci, [_vp, _u64p, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(_sz), _sz, _sz, _vp]),
     ("sa_fri_fold", _ci, [_vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
     ("sa_fri_round", _ci, [_vp, _vp, _vp, _sz, _u64p, _u64p, _u64p, _vp]),
@@ -951,21 +953,46 @@ class CudaEngine:
         self._count("h2d", host.numel())
         return host.to(self.device)
 
-    def verify_chunk(self, buf, L):
+    def transcript_bytes(self, shape):
+        """sa_transcript_bytes: one proof's workspace for a plan shape (SA_TRANSCRIPT_SHAPE ints), 0 if refused"""
+        return self.lib.sa_transcript_bytes((ctypes.c_uint64 * 10)(*shape))
+
+    def transcript_sections(self, buf, parts, L, nstat, nproofs, shape):
+        """sa_transcript_sections over the chunk VerifierPlan._transcript_chunk laid out: `buf` its uploaded uint8
+        tensor, parts the byte offsets of its proofs, proof_at, prefixes, statement and zerofier root, and
+        L["section_at"] the sections' byte offsets in include/sa_b200.h's order.  Returns the
+        zeroed-then-written sections (a uint8 tensor of L["bytes"]) and the per-proof out bytes (a uint8 tensor), no
+        synchronisation"""
+        torch = self.torch
+        sec = torch.zeros(max(L["bytes"], 16), dtype=torch.uint8, device=self.device)
+        out = torch.empty(80 * max(nproofs, 1), dtype=torch.uint8, device=self.device)
+        ws = torch.empty(max(self.transcript_bytes(shape) * nproofs, 16), dtype=torch.uint8, device=self.device)
+        ptr = buf.data_ptr()
+        at = (ctypes.c_uint64 * len(L["section_at"]))(*L["section_at"])
+        zroot = ptr + parts["zroot"] if shape[5] == shape[0] + 2 else None
+        self._check(self.lib.sa_transcript_sections(
+            sec.data_ptr(), at, out.data_ptr(), ws.data_ptr(), ptr + parts["proofs"], ptr + parts["proof_at"],
+            ptr + parts["prefixes"], ptr + parts["statement"], nstat, zroot, nproofs,
+            (ctypes.c_uint64 * 10)(*shape), self._stream()))
+        return sec, out
+
+    def verify_chunk(self, buf, L, extra=None):
         """The device checks of one chunk of proofs (DESIGN section 3.15) from `buf`, the chunk's one uploaded uint8
         tensor, whose sections start at the byte offsets of the layout L (sa_stark.VerifierPlan._pack):
         sa_merkle_verify_batch over L["paths"] paths, sa_fri_colinear_batch over L["colinear"] items,
         sa_verify_combination over L["k"] indices of L["proofs"] proofs, and for the proofs' last codewords one
         sa_merkle_tree_batch, one batched inverse sa_ntt and sa_poly_degree_batch.  Everything lands in one result
         buffer read with one download: (Merkle flags, colinearity flags, combination flags, the last codewords'
-        degrees, their tree roots as bytes)."""
+        degrees, their tree roots as bytes), and with `extra`, a uint8 device tensor read back in the same
+        download, its bytes last."""
         torch, st = self.torch, self._stream()
         lib = self.lib
         ptr = buf.data_ptr()
         at = lambda name: ptr + L[name]  # noqa: E731
         npath, ncol, B, k, m = L["paths"], L["colinear"], L["proofs"], L["k"], L["last_len"]
         nflag = npath + ncol + B * k
-        res = torch.empty(4 * nflag + 8 * B + 64 * B + 8, dtype=torch.uint8, device=self.device)
+        nextra = 0 if extra is None else extra.numel()
+        res = torch.empty(4 * nflag + 8 * B + 64 * B + 8 + nextra, dtype=torch.uint8, device=self.device)
         flags = res.data_ptr()
         deg_at = 4 * nflag + (-4 * nflag) % 8
         self._check(lib.sa_merkle_verify_batch(flags, at("roots"), at("leaves"), at("leaf_index"), at("depth"),
@@ -985,12 +1012,15 @@ class CudaEngine:
             coeffs = self.ntt(last.reshape(B * m, 2), m.bit_length() - 1, L["last_omega"], inverse=True, batch=B)
             self._check(lib.sa_poly_degree_batch(flags + deg_at, coeffs.data_ptr(), m, B, st))
             res[deg_at + 8 * B:deg_at + 72 * B].view(B, 64).copy_(trees[:, 1])
+        if nextra:
+            res[deg_at + 72 * B:deg_at + 72 * B + nextra].copy_(extra)
         host = res.cpu().numpy()
         self._count("d2h", res.numel())
         import numpy as np
-        return (host[:4 * npath].view(np.uint32), host[4 * npath:4 * (npath + ncol)].view(np.uint32),
-                host[4 * (npath + ncol):4 * nflag].view(np.uint32), host[deg_at:deg_at + 8 * B].view(np.int64),
-                host[deg_at + 8 * B:deg_at + 72 * B].tobytes())
+        got = (host[:4 * npath].view(np.uint32), host[4 * npath:4 * (npath + ncol)].view(np.uint32),
+               host[4 * (npath + ncol):4 * nflag].view(np.uint32), host[deg_at:deg_at + 8 * B].view(np.int64),
+               host[deg_at + 8 * B:deg_at + 72 * B].tobytes())
+        return got if extra is None else got + (host[deg_at + 72 * B:deg_at + 72 * B + nextra].tobytes(),)
 
     # ------------------------------------------------------------------ fri
     def fri_fold(self, vec, alpha, offset, omega):

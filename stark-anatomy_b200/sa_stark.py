@@ -43,8 +43,10 @@ os.urandom: the proof is the one the unseeded prover gives with os.urandom = ``s
 ``prove_plain``; ``disable()`` restores both.  Off by default, as ``sa_accel``.  Nothing here imports torch or holds
 device state outside a plan.
 """
+import hashlib
 import itertools
 import os
+import pickle
 from hashlib import blake2b
 
 import sa_host
@@ -845,6 +847,15 @@ LAST_FORM = "last codeword is not well formed"                                  
 COLINEAR = "colinearity check failure"                                             # fri.py:208
 MALFORMED = "malformed"
 CHUNK_BYTES = 1 << 30  # one chunk's device buffers, as coset_batch_max bounds a coset call's
+SECTIONS = ("roots", "leaves", "leaf_index", "depth", "digests", "path_offset", "ay", "by", "cy", "alpha", "items",
+            "proof_data", "last", "a_index", "round")  # _pack's order; sa_transcript_sections writes them in it
+# The device route reads a call's proofs when at least this many of them can take it.  Its fixed cost is one thread
+# parsing a whole proof (about 35 ms for a 1.1-1.3 MB signature), so below this count the host route is faster:
+# per signature, host / device route, FastRPSSS 13.2 / 13.8 ms at 4 and 12.5 / 9.7 ms at 6, RPSSS 8.6 / 10.1 ms
+# at 4 and 8.7 / 7.3 ms at 6 (H100 80GB HBM3 at a 700 W limit, tools/stark_verify.py, DESIGN section 3.17).
+DEVICE_ROUTE_MIN_PROOFS = 6
+TRANSCRIPT_PREFIX, TRANSCRIPT_OUT = 144, 80  # include/sa_b200.h's per-proof prefix and out strides
+_transcripts_checked = {}  # (shape, FieldElement class, pickle protocol) -> whether the stand-in check passed
 
 
 def _xor_exponent(e):
@@ -941,6 +952,8 @@ class VerifierPlan:
             else:
                 self.zcoef = eng.geo_zerofier(omicron, ncycles - 1)
         self._statements = {}
+        self.transcript = None
+        self.transcript = self._transcript_setup(eng)
 
     # -- the statement of one boundary: its zerofiers, interpolants and shifts (fast_stark.py:53-67, 272-277) --
     def _statement(self, boundary):
@@ -1112,19 +1125,23 @@ class VerifierPlan:
             add(name, sa_marshal.pack(vals))
         add("a_index", np.array(aidx, dtype=np.uint64).tobytes())
         add("round", np.array(rnd, dtype=np.uint32).tobytes())
-        stark = self.stark
-        L.update(paths=len(idx), colinear=len(ay), proofs=len(parsed), k=ktop, last_len=self.last_len,
-                 fri_offset=self.fri.offset.value, fri_omega=self.fri.omega.value, prog=self.prog, ncons=ncons,
-                 nregs=nregs, blen=blen, offset=stark.generator.value, omega=stark.omega.value, log_n=self.log_n,
-                 ef=self.ef, zcoef=self.zcoef,
-                 last_omega=pow(self.fri.omega.value, 1 << (rounds - 1), P))
+        self._constants(L, len(idx), len(ay), len(parsed), ktop, blen)
         return b"".join(sections), L
 
-    def _decide(self, pr, mflags, cflags, kflags, degree, root):
+    def _constants(self, L, npath, ncol, nproofs, ktop, blen):
+        """the layout's counts and the plan's constants verify_chunk reads beside the section offsets"""
+        stark = self.stark
+        L.update(paths=npath, colinear=ncol, proofs=nproofs, k=ktop, last_len=self.last_len,
+                 fri_offset=self.fri.offset.value, fri_omega=self.fri.omega.value, prog=self.prog,
+                 ncons=len(self.constraints), nregs=self.nregs, blen=blen, offset=stark.generator.value,
+                 omega=stark.omega.value, log_n=self.log_n, ef=self.ef, zcoef=self.zcoef,
+                 last_omega=pow(self.fri.omega.value, 1 << (self.rounds - 1), P))
+
+    def _decide(self, last_root, mflags, cflags, kflags, degree, root):
         """the reference's verdict from one proof's device flags, checks in the reference's order: (verdict, reason,
-        whether the zerofier vanished at the failing index)"""
+        whether the zerofier vanished at the failing index); last_root is the proof's last FRI root"""
         k, rounds = self.k, self.rounds
-        if root != pr.fri_roots[-1]:
+        if root != last_root:
             return False, LAST_FORM
         bound = self.last_len // self.ef - 1
         if degree > bound:
@@ -1154,12 +1171,14 @@ class VerifierPlan:
         npath = (self.rounds - 1) * 3 * self.k + sum(len(reads) for _, reads in pr.opened)
         ndigest = sum(len(p) for paths in pr.fri_paths for p in paths) + sum(
             len(p) for _, reads in pr.opened for _, _, p in reads)
-        ncol = (self.rounds - 1) * self.k
         blen, shifts, _ = pr.statement
-        ndata = len(pr.weights) + len(shifts) + 2 * self.nregs * blen
-        nitems = len(pr.top) * (4 + 2 * self.nregs)
+        return self._section_bytes(npath, ndigest, len(pr.top), len(pr.weights) + len(shifts) + 2 * self.nregs * blen)
+
+    def _section_bytes(self, npath, ndigest, ntop, ndata):
+        ncol = (self.rounds - 1) * self.k
+        nitems = ntop * (4 + 2 * self.nregs)
         return (npath * (64 + 16 + 8 + 4 + 8 + 4) + 64 * ndigest + ncol * (4 * 16 + 8 + 4 + 4) +
-                16 * (nitems + ndata) + 4 * len(pr.top) + self.last_len * (16 + 128 + 16) + 8 + 64 + 11 * 16)
+                16 * (nitems + ndata) + 4 * ntop + self.last_len * (16 + 128 + 16) + 8 + 64 + 11 * 16)
 
     def _chunks(self, parsed):
         """runs of consecutive proofs whose device buffers (_bytes) stay within CHUNK_BYTES; a proof above the bound
@@ -1181,16 +1200,28 @@ class VerifierPlan:
         prints for the first failing check (its three lines for the last codeword's degree), "leaf path" for an
         opened leaf's path, "combination" for the combination and "malformed" for a stream outside the shape.  A
         zero transition zerofier value at a checked index raises the reference's AssertionError("divide by zero")
-        with the proof's index as ``proof_index``, as verifying the proofs one at a time in order would."""
+        with the proof's index as ``proof_index``, as verifying the proofs one at a time in order would.
+
+        A proof whose bytes are the canonical pickle of a stream of the plan's shape, with a stream whose Fiat-Shamir
+        the device replays, is read on the device (the device route, DESIGN section 3.17) when the call has at least
+        DEVICE_ROUTE_MIN_PROOFS such proofs; every other proof is unpickled and packed on the host.  Both routes give
+        the same verdicts and exceptions."""
         proofs, boundaries = list(proofs), list(boundaries)
         B = len(proofs)
         assert len(boundaries) == B, "sa_stark: %d proofs and %d boundaries" % (B, len(boundaries))
         streams = [None] * B if proof_streams is None else list(proof_streams)
         assert len(streams) == B, "sa_stark: %d proofs and %d proof streams" % (B, len(streams))
+        eng = sa_engine.get_engine()
+        decided = self._verify_on_device(eng, proofs, boundaries, streams)  # b -> verdict or exception
         out = [None] * B
         parsed = []
         for b in range(B):
             try:
+                if b in decided:
+                    # what _parse raises for a stream it deserializes with enough objects, in the same order
+                    max(c for c, _, _ in boundaries[b])
+                    self._statement(boundaries[b])
+                    continue
                 pr = self._parse(proofs[b], boundaries[b], streams[b])
             except Exception as exc:
                 exc.proof_index = b
@@ -1199,7 +1230,6 @@ class VerifierPlan:
                 out[b] = (False, MALFORMED)
             else:
                 parsed.append((b, pr))
-        eng = sa_engine.get_engine()
         for chunk in self._chunks(parsed):
             raw, L = self._pack([pr for _, pr in chunk])
             mflags, cflags, kflags, degrees, roots = eng.verify_chunk(eng.upload_bytes(raw), L)
@@ -1208,14 +1238,206 @@ class VerifierPlan:
             for j, (b, pr) in enumerate(chunk):
                 nm = (self.rounds - 1) * 3 * self.k + sum(len(reads) for _, reads in pr.opened)
                 nc = (self.rounds - 1) * self.k
-                try:
-                    out[b] = self._decide(pr, mflags[m:m + nm], cflags[c:c + nc], kflags[q:q + ktop], degrees[j],
-                                          roots[64 * j:64 * (j + 1)])
-                except AssertionError as exc:
-                    exc.proof_index = b
-                    raise
+                decided[b] = self._outcome(pr.fri_roots[-1], mflags[m:m + nm], cflags[c:c + nc], kflags[q:q + ktop],
+                                           degrees[j], roots[64 * j:64 * (j + 1)])
                 m, c, q = m + nm, c + nc, q + ktop
+        for b in sorted(decided):
+            if isinstance(decided[b], BaseException):
+                decided[b].proof_index = b
+                raise decided[b]
+            out[b] = decided[b]
         return out if reasons else [v for v, _ in out]
+
+    def _outcome(self, *args):
+        try:
+            return self._decide(*args)
+        except AssertionError as exc:
+            return exc
+
+    # -- the device route (DESIGN section 3.17) --
+    def _transcript_counts(self, nopen):
+        k, rounds, log_n = self.k, self.rounds, self.log_n
+        fri_digests = sum(k * (3 * (log_n - r) - 1) for r in range(rounds - 1))
+        path_digests = fri_digests + 4 * nopen * k * log_n
+        nroots = self.nregs + 1 + rounds
+        nvalues = self.last_len + 3 * (rounds - 1) * k + 4 * nopen * k
+        npaths = 3 * (rounds - 1) * k + 4 * nopen * k
+        memo = 2 + 3 * (rounds - 1) * k + 4 * nopen * k + (rounds - 1) * k + nroots + path_digests + 2 * nvalues + 10
+        return npaths, path_digests, memo
+
+    def _transcript_setup(self, eng):
+        """the shape sa_transcript_sections reads this plan's proofs with, or None (the host route only): an engine
+        without the entry point, a shape it refuses, or a pickler whose output on a stand-in stream of the shape the
+        device does not read, or whose Fiat-Shamir prefixes it does not hash as pickle.dumps writes them"""
+        if not hasattr(eng, "transcript_sections") or self.rounds < 2 or self.k > self.last_len:
+            return None
+        shape = self._transcript_shape()
+        if eng.transcript_bytes(shape) == 0:
+            return None
+        key = (shape, sa_host.algebra.FieldElement, pickle.DEFAULT_PROTOCOL)
+        if key not in _transcripts_checked:
+            self.transcript = shape
+            _transcripts_checked[key] = self._transcript_check(eng)
+        return shape if _transcripts_checked[key] else None
+
+    def _transcript_shape(self):
+        """include/sa_b200.h's SA_TRANSCRIPT_SHAPE words for this plan at the running pickle protocol"""
+        nopen = self.nregs + 1 + (self.zerofier_root is not None)
+        W = 1 + 2 * len(self.constraints) + 2 * self.nregs
+        return (self.nregs, self.rounds, self.k, self.last_len, self.log_n, nopen, W, pickle.DEFAULT_PROTOCOL,
+                self.ef, self._transcript_counts(nopen)[2])
+
+    def _standin(self, seed=0):
+        """a stream of the plan's shape with random digests and elements of every int encoding's size"""
+        import random
+        rng = random.Random(seed)
+        field, FE = self.stark.field, sa_host.algebra.FieldElement
+        el = lambda: FE(rng.choice([rng.randrange(1 << 8), rng.randrange(1 << 16), rng.randrange(1 << 31),  # noqa
+                                    rng.randrange(P)]), field)
+        dg = lambda: rng.randbytes(64)  # noqa: E731
+        objs = [dg() for _ in range(self.nregs + 1 + self.rounds)] + [[el() for _ in range(self.last_len)]]
+        for r in range(self.rounds - 1):
+            objs += [(el(), el(), el()) for _ in range(self.k)]
+            objs += [[dg() for _ in range(self.log_n - r - (q % 3 == 2))] for q in range(3 * self.k)]
+        for _ in range(self.nregs + 1 + (self.zerofier_root is not None)):
+            for _ in range(4 * self.k):
+                objs += [el(), [dg() for _ in range(self.log_n)]]
+        return objs
+
+    def _transcript_check(self, eng):
+        """the stand-in's pickle is accepted, and its weights, alphas and indices are the ones the host draws from
+        shake_256(pickle.dumps(objects[:j]))"""
+        objs = self._standin()
+        fs = lambda j: hashlib.shake_256(pickle.dumps(objs[:j])).digest(32)  # noqa: E731
+        j0 = self.nregs + 1
+        weights = [w.value for w in self.stark.sample_weights(1 + 2 * len(self.constraints) + 2 * self.nregs, fs(j0))]
+        alphas = [self.stark.field.sample(fs(j0 + 1 + r)).value for r in range(self.rounds)]
+        top = self.fri.sample_indices(fs(j0 + self.rounds + 1), self.n >> 1, self.last_len, self.k)
+        stat = (1, [0] * (len(self.constraints) + self.nregs), [0] * (2 * self.nregs))
+        raw, parts, L, nstat = self._transcript_chunk([(pickle.dumps(objs), b"", stat)])
+        sec, out = eng.transcript_sections(eng.upload_bytes(raw), parts, L, nstat, 1, self.transcript)
+        sec, out = sec.cpu().numpy().tobytes(), out.cpu().numpy().tobytes()
+        fe = lambda name, n: [int.from_bytes(sec[L[name] + 16 * i:L[name] + 16 * (i + 1)], "little")  # noqa: E731
+                              for i in range(n)]
+        ncol = (self.rounds - 1) * self.k
+        aidx = [int.from_bytes(sec[L["a_index"] + 8 * i:L["a_index"] + 8 * (i + 1)], "little") for i in range(ncol)]
+        return (out[0] == 1 and fe("proof_data", len(weights)) == weights and
+                fe("alpha", ncol) == [a for a in alphas[:-1] for _ in range(self.k)] and
+                aidx == [i % (self.n >> (r + 1)) for r in range(self.rounds - 1) for i in top])
+
+    def _transcript_chunk(self, items):
+        """one device chunk's upload (the proofs, their offsets and prefixes, the statements at the chunk's blen and
+        the zerofier root), the byte offsets of its parts, the sections' layout L as _pack would give it, and the
+        statement elements per proof.  items: (proof bytes, prefix, statement or None)"""
+        nregs, k, B = self.nregs, self.k, len(items)
+        nopen = nregs + 1 + (self.zerofier_root is not None)
+        npaths, path_digests, _ = self._transcript_counts(nopen)
+        blen = max([st[0] for _, _, st in items if st is not None], default=1)
+        nstat = len(self.constraints) + nregs + 2 * nregs * blen
+        proofs, at, prefixes, stat = [], [], [], []
+        used = 0
+        for proof, prefix, st in items:
+            at += [used, len(proof)]
+            proofs.append(proof + bytes(-len(proof) % 16))
+            used += len(proof) + (-len(proof) % 16)
+            prefixes.append(len(prefix).to_bytes(8, "little") + bytes(8) + prefix[:128] +
+                            bytes(TRANSCRIPT_PREFIX - 16 - len(prefix[:128])))
+            if st is None:
+                stat += [0] * nstat
+                continue
+            blen_p, shifts, coef = st
+            stat += shifts
+            for s in range(nregs):
+                z, it = coef[2 * s * blen_p:(2 * s + 1) * blen_p], coef[(2 * s + 1) * blen_p:(2 * s + 2) * blen_p]
+                stat += z + [0] * (blen - blen_p) + it + [0] * (blen - blen_p)
+        import numpy as np
+        parts = {}
+        chunks = []
+        for name, raw in (("proofs", b"".join(proofs)), ("proof_at", np.array(at, dtype=np.uint64).tobytes()),
+                          ("prefixes", b"".join(prefixes)), ("statement", sa_marshal.pack(stat)),
+                          ("zroot", self.zerofier_root or b"")):
+            parts[name] = sum(len(c) for c in chunks)
+            chunks.append(raw + bytes(-len(raw) % 16))
+        W = 1 + 2 * len(self.constraints) + 2 * nregs
+        ncol = (self.rounds - 1) * k
+        sizes = {"roots": 64 * npaths, "leaves": 16 * npaths, "leaf_index": 8 * npaths, "depth": 4 * npaths,
+                 "digests": 64 * path_digests, "path_offset": 8 * npaths, "ay": 16 * ncol, "by": 16 * ncol,
+                 "cy": 16 * ncol, "alpha": 16 * ncol, "items": 16 * 2 * k * (4 + 2 * nregs),
+                 "proof_data": 16 * (W + nstat), "last": 16 * self.last_len, "a_index": 8 * ncol, "round": 4 * ncol}
+        L, size = {}, 0
+        for name in SECTIONS:
+            L[name] = size
+            size += B * sizes[name] + (-B * sizes[name]) % 16
+        L["bytes"] = size
+        L["section_at"] = [L[name] for name in SECTIONS]
+        self._constants(L, B * npaths, B * ncol, B, 2 * k, blen)
+        return b"".join(chunks), parts, L, nstat
+
+    @staticmethod
+    def _fs_prefix(stream):
+        """the bytes the stream's verifier_fiat_shamir hashes before pickle.dumps(objects[:read_index]), or None
+        where a stand-in transcript of two objects shows it hashes something else"""
+        try:
+            q = (stream if stream is not None else sa_host.ip.ProofStream()).deserialize(
+                pickle.dumps([bytes(64), bytes(range(64))]))
+            q.pull()
+            q.pull()
+            prefix = getattr(q, "prefix", b"")
+            if type(prefix) is not bytes or len(prefix) > 128:
+                return None
+            if q.verifier_fiat_shamir() != hashlib.shake_256(prefix + pickle.dumps(q.objects[:2])).digest(32):
+                return None
+            return prefix
+        except Exception:
+            return None
+
+    def _verify_on_device(self, eng, proofs, boundaries, streams):
+        """the device route: {b: verdict or exception} for the proofs the device read; the others are left to the
+        host route.  Chunks of consecutive such proofs, each within CHUNK_BYTES, one upload, six transcript launches,
+        verify_chunk's ladder and one download each"""
+        if self.transcript is None:
+            return {}
+        nopen = self.nregs + 1 + (self.zerofier_root is not None)
+        npaths, path_digests, _ = self._transcript_counts(nopen)
+        base = eng.transcript_bytes(self.transcript) + TRANSCRIPT_PREFIX + TRANSCRIPT_OUT + 16
+        W = 1 + 2 * len(self.constraints) + 2 * self.nregs
+        eligible = []
+        for b, proof in enumerate(proofs):
+            prefix = self._fs_prefix(streams[b]) if type(proof) is bytes else None
+            if prefix is not None:
+                eligible.append((b, proof, prefix))
+        if len(eligible) < DEVICE_ROUTE_MIN_PROOFS:
+            return {}
+        chunks, cur, used = [], [], 0
+        for b, proof, prefix in eligible:
+            try:
+                max(c for c, _, _ in boundaries[b])
+                st = self._statement(boundaries[b])
+            except Exception:
+                st = None  # the walk in verify_batch raises it where the host route would
+            blen = st[0] if st is not None else 1
+            size = len(proof) + base + self._section_bytes(npaths, path_digests, 2 * self.k,
+                                                           W + len(self.constraints) + self.nregs + 2 * self.nregs * blen)
+            if cur and used + size > CHUNK_BYTES:
+                chunks.append(cur)
+                cur, used = [], 0
+            cur.append((b, proof, prefix, st))
+            used += size
+        chunks += [cur] if cur else []
+        decided = {}
+        nm, nc = npaths, (self.rounds - 1) * self.k
+        ktop = 2 * self.k
+        for chunk in chunks:
+            raw, parts, L, nstat = self._transcript_chunk([(p, x, st) for _, p, x, st in chunk])
+            sec, out = eng.transcript_sections(eng.upload_bytes(raw), parts, L, nstat, len(chunk), self.transcript)
+            mflags, cflags, kflags, degrees, roots, out = eng.verify_chunk(sec, L, extra=out)
+            for j, (b, _, _, _) in enumerate(chunk):
+                if out[TRANSCRIPT_OUT * j] != 1:
+                    continue
+                last_root = bytes(out[TRANSCRIPT_OUT * j + 16:TRANSCRIPT_OUT * (j + 1)])
+                decided[b] = self._outcome(last_root, mflags[j * nm:(j + 1) * nm], cflags[j * nc:(j + 1) * nc],
+                                           kflags[j * ktop:(j + 1) * ktop], degrees[j], roots[64 * j:64 * (j + 1)])
+        return decided
 
     def verify(self, proof, boundary, proof_stream=None):
         """verify_batch of one proof: its bool"""
